@@ -5,6 +5,7 @@ of that architecture), 1024-in / 128-out, batch 32, on N GPUs of one node (N>1 =
 One "step" = one pass of the hot path over one batch: prefill of B x 1024 prompt tokens + 128 greedy tokens.
 
     python bench.py --gpus 1 --steps 5 --warmup 3              # this repo's CUDA path
+    python bench.py --gpus 1 --steps 5 --warmup 3 --dump-outputs DIR   # + the last timed step's output ids as DIR/*.npy
     python bench.py --impl reference --gpus 1 --steps 2        # the reference's HF-transformers CPU backend
     torchrun --nproc-per-node N ... bench.py --gpus N ...      # TP=N over NCCL
 
@@ -50,7 +51,8 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sustained=d["bf16_tflops_sustained"], src="measured")
-    return dict(hbm_gbs=6650.0, tf_burst=1590.0, tf_sustained=1400.0, src="fallback")
+    # NVIDIA's H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 dense bf16 TFLOP/s -- denominators, not reached figures
+    return dict(hbm_gbs=3350.0, tf_burst=989.0, tf_sustained=989.0, src="H100 SXM data sheet")
 
 
 def algorithmic(cfg, B, S_in, S_out, tp=1):
@@ -71,35 +73,8 @@ def algorithmic(cfg, B, S_in, S_out, tp=1):
                 kv_bytes_per_token=kv_per_tok, layer_params=layer_params)
 
 
-def ncu_decode_traffic(cfg, B, S_in, S_out, tp):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one decode step, assembled from the committed `ncu --set full`
-    captures (profiles/r02_ncu_full_summary.json: one launch per decode kernel at B=32, ctx ~1024; the LM-head launch from
-    the round-1 capture of the unchanged kernel) times the launches per step.  Only meaningful for the configuration the
-    capture was taken on; None otherwise."""
-    if tp != 1 or B != 32 or cfg is not LLAMA3_8B or S_in != 1024:
-        return None
-    try:
-        def gb(e):
-            def f(v):
-                x, unit = v.split()
-                return float(x) * {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}[unit]
-            return f(e["dram__bytes_read.sum"]) + f(e["dram__bytes_write.sum"])
-        rows = json.load(open(os.path.join(ROOT, "profiles", "r02_ncu_full_summary.json")))
-        r01 = json.load(open(os.path.join(ROOT, "profiles", "r01_final_ncu_full_summary.json")))
-        dec = [e for e in rows if e["report"] == "r02_gemm_decode"]
-        lm_head = next(gb(e) for e in r01 if e["report"] == "r01f_gemm_decode" and "gemm_tn_kernel<32, 3>" in e["kernel"])
-        gate_up = next(gb(e) for e in dec if "gemm_tn_kernel<32, 4>" in e["kernel"])
-        parts = sorted(gb(e) for e in dec if "gemm_tn_kernel<32, 5>" in e["kernel"])   # o (34 MB) < qkv (51 MB) < down (118 MB)
-        o_proj, qkv, down = parts[0], parts[1], parts[-1]
-        attn = next(gb(e) for e in rows if "attn_decode_kernel" in e["kernel"])
-        L = cfg["num_hidden_layers"]
-        return int(L * (qkv + o_proj + gate_up + down + attn) + lm_head)
-    except Exception:
-        return None
-
-
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region (the card's power limit bounds its sustained clocks)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -387,7 +362,7 @@ def run_b200(args):
         torch.cuda.synchronize()
 
     # ---- device-resident timing: prompt staged once, K x (prefill + T-1 decode steps), CUDA events on the
-    # engine stream; weights (16 GB) >> L2 (126 MB) so every step re-reads HBM.
+    # engine stream; weights (16 GB) >> L2 (50 MB) so every step re-reads HBM.
     eng.stage(ids, None, max_new_tokens=T, pad_token_id=pad)
     for _ in range(args.warmup):
         eng.run_staged_timed(T - 1)
@@ -406,6 +381,11 @@ def run_b200(args):
     clocks = sampler.stop() if rank == 0 else None
     out = eng.fetch_staged()
     assert out.shape == (B, S + T), out.shape
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        # what a caller of the timed path receives from its last step: prompt + greedy ids [B, S + T] (float64: exact ids)
+        np.save(os.path.join(args.dump_outputs, "output_ids.npy"), out.cpu().numpy().astype(np.float64))
     dev_ms = sum(pre) + sum(dec)
     tm = torch.tensor([dev_ms, statistics.median(pre), sum(dec)], dtype=torch.float64, device=dev)
     if world > 1:
@@ -484,7 +464,7 @@ def run_b200(args):
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": round(ms_per_step, 3), "higher_is_better": True,
         "scaling": "strong", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
         "config": workload_config(model_name, B, S, T, world),
-        "notes": {"l2": f"weights {alg['weight_bytes'] / 1e9:.1f} GB per GPU >> 126 MB L2: no flush needed",
+        "notes": {"l2": f"weights {alg['weight_bytes'] / 1e9:.1f} GB per GPU >> 50 MB L2: no flush needed",
                   "timer": "CUDA events on the engine stream, max over ranks"},
         "parity_check": parity,
         "full_size_checks": checks,
@@ -500,9 +480,7 @@ def run_b200(args):
         "clocks": clocks,
         "roofline": {"kernel": "decode step: gemm_tn_kernel<swap-AB> weight streaming + attn_decode KV read",
                      "bound": "hbm", "achieved": round(ach_gbs, 1), "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                     "frac": round(ach_gbs / peaks["hbm_gbs"], 4), "traffic": ncu_decode_traffic(cfg, B, S, T, world),
-                     "traffic_src": "ncu --set full per-launch dram bytes x launches per step (profiles/r02_ncu_full_summary.json); "
-                                    "null off the captured configuration", "peak_src": peaks["src"],
+                     "frac": round(ach_gbs / peaks["hbm_gbs"], 4), "peak_src": peaks["src"],
                      "algorithmic_bytes_per_launch": int(alg["decode_bytes_per_step"])},
         "roofline_prefill": {"kernel": "prefill: gemm_tn_kernel<256> + attn_prefill", "bound": "tensor",
                              "achieved": round(ach_tf, 1), "peak": peaks["tf_sustained"], "unit": "TFLOP/s",
@@ -547,7 +525,12 @@ def main():
                     help="--impl reference: CPU seconds the whole --steps/--warmup run may take before the sample is shortened")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity-check", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the output ids of the last timed step to DIR/output_ids.npy (float64)")
     args = ap.parse_args()
+    if args.impl == "reference" and args.dump_outputs:
+        # the reference arm times one sequence on the CPU with its own weights: its ids are not the GPU arm's workload
+        ap.error("--dump-outputs writes the GPU arm's outputs; it does not apply to --impl reference")
     if args.impl == "reference":
         run_reference(args)
     else:

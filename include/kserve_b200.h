@@ -1,5 +1,5 @@
 /*
- * kserve_b200 — C ABI of the B200-native LLM predict path.
+ * kserve_b200 — C ABI of the H100-native LLM predict path.
  *
  * This is the drop-in boundary for the reference's HF generative runtime: every entry point below
  * replaces one call the reference makes into its third-party compute backend (transformers/torch) or,
@@ -176,7 +176,7 @@ int b200_op_attn_prefill(const void* q, int64_t ldq, void* out, int64_t ldo, con
                          const void* vcache, const int32_t* page_table, int max_pages,
                          const int32_t* cu_seqlens, const int32_t* seq_slot, int B, int max_len, int nh, int nkv,
                          void* stream);
-/* tcgen05/TMEM prefill attention (the engine's default); q_rows = rows of the q buffer, num_pages = pages of the caches */
+/* wgmma prefill attention (the engine's default); q_rows = rows of the q buffer, num_pages = pages of the caches */
 int b200_op_attn_prefill_tc(const void* q, int64_t ldq, int q_rows, void* out, int64_t ldo, const void* kcache,
                             const void* vcache, int num_pages, const int32_t* page_table, int max_pages,
                             const int32_t* cu_seqlens, const int32_t* seq_slot, int B, int max_len, int nh, int nkv,

@@ -1,7 +1,7 @@
 """`python -m kserve_b200 --model_dir /mnt/models --model_name llama` — the entrypoint that replaces
 `python -m huggingfaceserver --backend huggingface` (python/huggingfaceserver/huggingfaceserver/__main__.py:60-345)
 for Llama-family decoders: same --model_id/--model_dir/--model_name/--max_model_len/--dtype flags, backend fixed to
-the B200 engine (no vLLM / transformers dispatch), plus --tensor_parallel_size (one process per GPU under torchrun)."""
+the H100 engine (no vLLM / transformers dispatch), plus --tensor_parallel_size (one process per GPU under torchrun)."""
 import argparse
 import os
 import sys
@@ -16,7 +16,7 @@ def main(argv=None):
     parser.add_argument("--model_id", default=None, help="alias of --model_dir (no Hub access in this runtime)")
     parser.add_argument("--max_model_len", "--max_length", type=int, default=None)
     parser.add_argument("--dtype", default="auto", choices=["auto", "float16", "float32", "bfloat16", "float", "half"],
-                        help="the reference's choices (__main__.py:195-210); the B200 engine computes in bfloat16, which is what "
+                        help="the reference's choices (__main__.py:195-210); the H100 engine computes in bfloat16, which is what "
                              "'auto' and 'bfloat16' select — the other values are refused at start-up rather than silently "
                              "served at a different precision")
     parser.add_argument("--backend", default="b200", choices=["b200"])
@@ -35,7 +35,7 @@ def main(argv=None):
     parser.add_argument("--max-latency", "--max_latency", dest="max_latency", type=int, default=5000)
     args, _ = parser.parse_known_args(argv)
     if args.dtype not in ("auto", "bfloat16"):
-        parser.error(f"--dtype {args.dtype}: the B200 runtime computes in bfloat16 only (use --dtype auto or bfloat16)")
+        parser.error(f"--dtype {args.dtype}: the H100 runtime computes in bfloat16 only (use --dtype auto or bfloat16)")
     if args.enable_batcher and (args.max_batchsize <= 0 or args.max_latency <= 0):
         parser.error("Invalid max batch size / max latency")        # cmd/agent/main.go:256-273
     from .generative_model import B200GenerativeModel

@@ -1,4 +1,4 @@
-"""In-tree build of the sm_100a shared library (nvcc cross-compiles without a GPU).
+"""In-tree build of the sm_90a shared library (nvcc cross-compiles without a GPU).
 
     python -m kserve_b200.build [--force]
 
@@ -16,7 +16,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libkserve_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared", "-diag-suppress", "177",
 ]
 SOURCES = ["engine.cu"]

@@ -1,14 +1,14 @@
-// Causal prefill attention on the 5th-generation tensor cores (tcgen05 + TMEM), SURVEY.md §8a row 15.
+// Causal prefill attention on the Hopper tensor cores (wgmma), SURVEY.md §8a row 15.
 //
-// One CTA = 128 query rows of one (sequence, head); KV is consumed in tiles of 64 tokens (= one page); two CTAs per SM.
-//   warp 0   : TMA producer — Q once, then K / V tiles into 2-stage 128B-swizzled rings straight from the paged
-//              cache (tensor map over [page*nkv*64 rows][128 dims], two 8 KB boxes per tile)
-//   warp 1   : MMA issuer — S = Q K^T  (tcgen05.mma M=128 N=64, both operands K-major, S in TMEM, double buffered)
-//                           O += P V   (A = P from shared memory, B = V as an MN-major operand, O accumulates in TMEM)
-//   warps 2-5: softmax — one thread per query row reads its S row with tcgen05.ld (no shuffles), online softmax in
-//              the log2 domain with *lazy* rescaling (O is only rescaled in TMEM when the running max grew by more
-//              than 2^8), writes P (bf16) into the swizzled A-operand layout, finally normalises O and stores bf16.
-// S_{j+1} = Q K_{j+1}^T is issued before the softmax of tile j finishes, so the tensor pipe overlaps the exp2 work.
+// One CTA = 128 query rows of one (sequence, head); KV is consumed in tiles of 64 tokens (= one page).
+//   warpgroup 0    : TMA producer — Q once, then K / V tiles into 2-stage 128B-swizzled rings straight from the paged
+//                    cache (tensor map over [page*nkv*64 rows][128 dims], two 8 KB boxes per tile)
+//   warpgroups 1-2 : 64 query rows each — S = Q K^T (wgmma m64n64k16, both operands K-major from shared memory, S in
+//                    registers), online softmax in the log2 domain on the register fragment (a row is spread over the
+//                    4 threads of a quad), then O += P V (wgmma m64n128k16 with P as the register A operand — the S
+//                    fragment layout is the A fragment layout, so P never goes through shared memory — and V as an
+//                    MN-major shared-memory operand), finally O / l stored as bf16.
+// The two consumer warpgroups run independently, so one's softmax overlaps the other's tensor-core work.
 #pragma once
 #include "common.cuh"
 #include "ops.cuh"
@@ -18,12 +18,9 @@ namespace b200 {
 constexpr int kTcQ = 128;                    // query rows per CTA
 constexpr int kTcKv = 64;                    // KV tokens per tile == one page
 constexpr int kTcTile = 128 * 64 * 2;        // one [128 x 64] bf16 swizzled tile = 16 KB (a K or V stage: two [64 x 64] boxes)
-// Q 2 tiles + K ring 2 stages + V ring 2 stages + P 1 tile = 112 KB (+ barriers): TWO CTAs per SM (2 x 256 TMEM columns), so
-// one CTA's tensor-core work overlaps the other CTA's softmax.  (r01: 128-token KV tiles, 192 KB, one CTA per SM, one
-// softmax pass blocking the tensor pipe: 18 % tensor-pipe active.)  The dynamic shared memory base is 1024-byte aligned
-// by declaration — there is no room for alignment slack with two CTAs per SM.
-constexpr int kTcSmem = 2 * kTcTile /*Q*/ + 2 * kTcTile /*K ring*/ + 2 * kTcTile /*V ring*/ + kTcTile /*P*/ + 256;
-constexpr int kTcThreads = 192;
+// Q 2 tiles + K ring 2 stages + V ring 2 stages = 96 KB, + alignment slack and barriers; one CTA per SM
+constexpr int kTcSmem = 2 * kTcTile /*Q*/ + 2 * kTcTile /*K ring*/ + 2 * kTcTile /*V ring*/ + 1024 + 256;
+constexpr int kTcThreads = 384;
 
 struct AttnTcParams {
   bf16* out; long long ldo;
@@ -37,89 +34,44 @@ struct AttnTcParams {
   const int32_t* kv_off;
 };
 
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
-      "%30,%31,%32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// MN-major (B = V[token][dim], dims contiguous) 128B-swizzled operand: 8 token rows x 128 B form one swizzle atom,
-// atoms along K (tokens) are SBO = 1024 B apart, the second 64-dim block of N is LBO = one 16 KB tile further.
-__device__ __forceinline__ uint64_t make_smem_desc_sw128_mn(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// kind::f16, D = f32, A = bf16 K-major, B = bf16 with selectable major-ness
-__host__ __device__ constexpr uint32_t make_idesc_bf16_bmn(int M, int N, int b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)b_mn << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-__global__ void __launch_bounds__(kTcThreads, 2)
+__global__ void __launch_bounds__(kTcThreads, 1)
 attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                        const __grid_constant__ CUtensorMap tmap_v, const AttnTcParams p) {
   TraceScope _ts(TK_ATTN_PREFILL);
-  extern __shared__ __align__(1024) uint8_t smem[];
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;                       // 2 tiles (dims 0-63 | 64-127), 128 rows each
   uint8_t* sK = sQ + 2 * kTcTile;           // ring[2] x {dims 0-63 | 64-127} x 64 tokens
   uint8_t* sV = sK + 2 * kTcTile;           // ring[2], same shape
-  uint8_t* sP = sV + 2 * kTcTile;           // [128 rows x 64 tokens]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + kTcTile);
-  uint64_t *q_full = bars, *k_full = bars + 1, *k_empty = bars + 3, *v_full = bars + 5, *v_empty = bars + 7,
-           *s_full = bars + 9, *s_empty = bars + 11, *p_full = bars + 13, *pv_done = bars + 14;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 15);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * kTcTile);
+  uint64_t *q_full = bars, *k_full = bars + 1, *k_empty = bars + 3, *v_full = bars + 5, *v_empty = bars + 7;
 
   const int b = blockIdx.z, h = blockIdx.y, qt = blockIdx.x;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   pdl_launch_dependents();
   pdl_wait();
   const int tok0 = p.cu_seqlens[b];
   const int len = p.cu_seqlens[b + 1] - tok0;
   const int q0 = qt * kTcQ;
   if (q0 >= len) return;
-  if ((smem_u32(smem) & 1023u) != 0) {
-    if (threadIdx.x == 0) printf("b200: attention shared memory base is not 1024-byte aligned\n");
-    __trap();
-  }
   const int kvh = h / (p.nh / p.nkv);
   const int32_t* pages = p.page_table + (long long)p.seq_slot[b] * p.max_pages;
   const int off_tiles = p.kv_off ? (p.kv_off[b] >> 7) : 0;    // 128-token blocks that precede this chunk's first query row
   const int ntiles = 2 * (off_tiles + qt + 1);                 // causal: 64-token KV tiles 0 .. 2 * (off_tiles + qt) + 1
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_q); tma_prefetch_desc(&tmap_k); tma_prefetch_desc(&tmap_v);
     mbar_init(q_full, 1);
     for (int i = 0; i < 2; ++i) {
-      mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 1);
-      mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], 1);
-      mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], 128);
+      mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 2);   // one arrival per consumer warpgroup
+      mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], 2);
     }
-    mbar_init(p_full, 128);
-    mbar_init(pv_done, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 256);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_s = tmem_base;          // S buffers: columns [0,64) and [64,128)
-  const uint32_t tmem_o = tmem_base + 128;    // O: columns [128,256)
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    if (threadIdx.x == 0) {
       mbar_arrive_expect_tx(q_full, 2 * kTcTile);
       tma_load_2d(sQ, &tmap_q, q_full, h * kHeadDim, tok0 + q0, kEvictNormal);
       tma_load_2d(sQ + kTcTile, &tmap_q, q_full, h * kHeadDim + 64, tok0 + q0, kEvictNormal);
@@ -139,157 +91,106 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
         tma_load_2d(vd + kTcTile / 2, &tmap_v, &v_full[st], 64, row0, kEvictLast);
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc_bf16_bmn(128, 64, 0);
-      constexpr uint32_t idesc_o = make_idesc_bf16_bmn(128, 128, 1);
-      mbar_wait(q_full, 0);
-      auto issue_s = [&](int j) {
-        const int buf = j & 1;
-        const uint32_t ph = (j >> 1) & 1;
-        mbar_wait(&s_empty[buf], ph ^ 1);
-        mbar_wait(&k_full[buf], ph);
-        tcgen05_fence_after();
-        const uint32_t kq = smem_u32(sQ), kk = smem_u32(sK + buf * kTcTile);
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16(tmem_s + buf * 64, make_smem_desc_sw128(kq + hh * kTcTile) + 2 * k,
-                      make_smem_desc_sw128(kk + hh * (kTcTile / 2)) + 2 * k, idesc_s, (hh | k) ? 1u : 0u);
-        umma_commit(&k_empty[buf]);
-        umma_commit(&s_full[buf]);
-      };
-      issue_s(0);
-      for (int j = 0; j < ntiles; ++j) {
-        if (j + 1 < ntiles) issue_s(j + 1);
-        const int st = j & 1;
-        mbar_wait(p_full, j & 1);
-        mbar_wait(&v_full[st], (j >> 1) & 1);
-        tcgen05_fence_after();
-        const uint32_t pa = smem_u32(sP), vb = smem_u32(sV + st * kTcTile);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {       // 16 tokens per MMA
-          const uint64_t adesc = make_smem_desc_sw128(pa) + 2 * k;
-          const uint64_t bdesc = make_smem_desc_sw128_mn(vb + (k * 16) * 128, kTcTile / 2);
-          umma_bf16(tmem_o, adesc, bdesc, idesc_o, (j > 0 || k > 0) ? 1u : 0u);
-        }
-        umma_commit(&v_empty[st]);
-        umma_commit(pv_done);
-      }
-    }
-    __syncwarp();
-  } else {
-    // ------------------------------------------------------------------ softmax / correction / epilogue
-    const int q = warp & 3;
-    const int r = q * 32 + lane;               // row of the tile handled by this thread
-    const int qrow = q0 + r;                   // row inside this chunk (bounds / output row)
-    const int qpos = off_tiles * 128 + qrow;   // position in the sequence (causal mask)
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    float m_ref = -INFINITY, l_run = 0.f;
-    for (int j = 0; j < ntiles; ++j) {
-      const int buf = j & 1;
-      mbar_wait(&s_full[buf], (j >> 1) & 1);
-      tcgen05_fence_after();
-      const bool diag = (j >= ntiles - 2);
-      // one TMEM pass: the 64 raw scores of this row stay in registers; the softmax scale is folded into the exponent
-      // (max on the raw scores — the scale is positive — then p = exp2(fma(s, scale, -m)): one FFMA per element)
-      float sv[64];
-      {
-        uint32_t sr[32];
-        tmem_ld_32x32(tmem_s + lane_base + buf * 64, sr);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) sv[i] = __uint_as_float(sr[i]);
-        tmem_ld_32x32(tmem_s + lane_base + buf * 64 + 32, sr);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) sv[32 + i] = __uint_as_float(sr[i]);
-      }
-      tcgen05_fence_before();
-      mbar_arrive(&s_empty[buf]);      // S[buf] is in registers: the next QK^T may overwrite it
-      float mx = -INFINITY;
-      if (diag) {
-#pragma unroll
-        for (int i = 0; i < 64; ++i) {
-          if (j * kTcKv + i > qpos) sv[i] = -INFINITY;
-          mx = fmaxf(mx, sv[i]);
-        }
-      } else {
-#pragma unroll
-        for (int i = 0; i < 64; ++i) mx = fmaxf(mx, sv[i]);
-      }
-      const float m_new = fmaxf(m_ref, mx * p.scale_log2);      // finite from tile 0 on: key 0 is visible to every row
-      // lazy rescale: keep the reference max unless it would let exp2 grow past 2^8
-      const bool grow = (m_ref == -INFINITY) || (m_new > m_ref + 8.0f);
-      const float corr = grow ? ((m_ref == -INFINITY) ? 0.f : exp2f(m_ref - m_new)) : 1.0f;
-      if (grow) m_ref = m_new;
-      if (j > 0) {
-        mbar_wait(pv_done, (j - 1) & 1);           // O (and the P buffer) are no longer in use by PV_{j-1}
-        tcgen05_fence_after();
-        if (__any_sync(0xffffffffu, grow)) {
-#pragma unroll 1
-          for (int c0 = 0; c0 < 128; c0 += 32) {
-            uint32_t orr[32];
-            tmem_ld_32x32(tmem_o + lane_base + c0, orr);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) orr[i] = __float_as_uint(__uint_as_float(orr[i]) * corr);
-            tmem_st_32x32(tmem_o + lane_base + c0, orr);
-          }
-          tmem_st_wait();
-        }
-      }
-      l_run *= corr;
-      // p = exp2(s - m_ref), row sum, bf16 P into the swizzled A-operand layout (one 128-byte row per query row)
-      uint8_t* prow = sP + r * 128;
-#pragma unroll
-      for (int g8 = 0; g8 < 8; ++g8) {
-        float pv[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          pv[i] = exp2f(fmaf(sv[8 * g8 + i], p.scale_log2, -m_ref));
-          l_run += pv[i];
-        }
-        uint4 o;
-        o.x = pack_bf16x2(pv[0], pv[1]); o.y = pack_bf16x2(pv[2], pv[3]);
-        o.z = pack_bf16x2(pv[4], pv[5]); o.w = pack_bf16x2(pv[6], pv[7]);
-        *reinterpret_cast<uint4*>(prow + ((g8 ^ (r & 7)) << 4)) = o;
-      }
-      tcgen05_fence_before();
-      fence_proxy_async_smem();        // P (generic-proxy stores) visible to the tensor core's async proxy
-      mbar_arrive(p_full);
-    }
-    // epilogue: O / l -> bf16
-    mbar_wait(pv_done, (ntiles - 1) & 1);
-    tcgen05_fence_after();
-    const float inv = 1.0f / l_run;
-    const bool valid = qrow < len;
-    bf16* orow = p.out + (long long)(tok0 + qrow) * p.ldo + h * kHeadDim;
-#pragma unroll 1
-    for (int c0 = 0; c0 < 128; c0 += 32) {
-      uint32_t orr[32];
-      tmem_ld_32x32(tmem_o + lane_base + c0, orr);
-      tmem_ld_wait();
-      if (valid) {
-#pragma unroll
-        for (int g8 = 0; g8 < 4; ++g8) {
-          uint4 o;
-          o.x = pack_bf16x2(__uint_as_float(orr[8 * g8 + 0]) * inv, __uint_as_float(orr[8 * g8 + 1]) * inv);
-          o.y = pack_bf16x2(__uint_as_float(orr[8 * g8 + 2]) * inv, __uint_as_float(orr[8 * g8 + 3]) * inv);
-          o.z = pack_bf16x2(__uint_as_float(orr[8 * g8 + 4]) * inv, __uint_as_float(orr[8 * g8 + 5]) * inv);
-          o.w = pack_bf16x2(__uint_as_float(orr[8 * g8 + 6]) * inv, __uint_as_float(orr[8 * g8 + 7]) * inv);
-          *reinterpret_cast<uint4*>(orow + c0 + 8 * g8) = o;
-        }
-      }
-    }
+    return;
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, 256);
+
+  // ------------------------------------------------------------------ consumers: softmax + both MMAs
+  const int half = wg - 1;                                        // query rows 64 * half ... + 63 of the tile
+  const int t = threadIdx.x - 128 * wg;
+  const int r_lo = 64 * half + 16 * (warp & 3) + (lane >> 2);     // this thread's fragment rows r_lo, r_lo + 8
+  const int qpos_lo = off_tiles * 128 + q0 + r_lo;                // position of row r_lo in the sequence (causal mask)
+  const int col_t = 2 * (lane & 3);                               // fragment column offset inside each 8-column group
+  float o[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  const uint32_t sq = smem_u32(sQ) + half * 64 * 128;
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < ntiles; ++j) {
+    const int st = j & 1;
+    const uint32_t ph = (j >> 1) & 1;
+    // ---- S = Q K^T
+    float s[32];
+    mbar_wait(&k_full[st], ph);
+    {
+      const uint32_t kk = smem_u32(sK + st * kTcTile);
+      wgmma_fence();
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_ss_n64(s, make_smem_desc_sw128(sq + hh * kTcTile) + 2 * k, make_smem_desc_sw128(kk + hh * (kTcTile / 2)) + 2 * k,
+                       (hh | k) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_keep(s);
+    }
+    if (t == 0) mbar_arrive(&k_empty[st]);
+    // ---- online softmax; the softmax scale is folded into the exponent (max on the raw scores — the scale is
+    // positive — then p = exp2(fma(s, scale, -m)): one FFMA per element)
+    if (j >= ntiles - 2) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int key = j * kTcKv + 8 * (i >> 2) + col_t + (i & 1);
+        if (key > qpos_lo + 8 * ((i >> 1) & 1)) s[i] = -INFINITY;
+      }
+    }
+    float corr[2];
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+        if (((i >> 1) & 1) == rr) mx = fmaxf(mx, s[i]);
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[rr], mx * p.scale_log2);   // finite from tile 0 on: key 0 is visible to every row
+      corr[rr] = (m_run[rr] == -INFINITY) ? 0.f : exp2f(m_run[rr] - m_new);
+      m_run[rr] = m_new;
+      l_run[rr] *= corr[rr];
+    }
+    uint32_t pa[16];
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const int rr = (i >> 1) & 1;
+      const float p0 = exp2f(fmaf(s[i], p.scale_log2, -m_run[rr]));
+      const float p1 = exp2f(fmaf(s[i + 1], p.scale_log2, -m_run[rr]));
+      l_run[rr] += p0 + p1;
+      pa[i >> 1] = pack_bf16x2(p0, p1);
+    }
+#pragma unroll
+    for (int i = 0; i < 64; ++i) o[i] *= corr[(i >> 1) & 1];
+    // ---- O += P V: 16 tokens per MMA; the S fragment of tokens [16k, 16k + 16) is the A fragment {pa[4k] .. pa[4k + 3]}
+    mbar_wait(&v_full[st], ph);
+    {
+      const uint32_t vb = smem_u32(sV + st * kTcTile);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint32_t a[4] = {pa[4 * k], pa[4 * k + 1], pa[4 * k + 2], pa[4 * k + 3]};
+        wgmma_rs_n128_tb(o, a, make_smem_desc_sw128_mn(vb + (k * 16) * 128, kTcTile / 2), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_keep(o);
+    }
+    if (t == 0) mbar_arrive(&v_empty[st]);
+  }
+  // epilogue: O / l -> bf16
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    l_run[rr] += __shfl_xor_sync(0xffffffffu, l_run[rr], 1);
+    l_run[rr] += __shfl_xor_sync(0xffffffffu, l_run[rr], 2);
+  }
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    const int qrow = q0 + r_lo + 8 * rr;
+    if (qrow >= len) continue;
+    const float inv = 1.0f / l_run[rr];
+    bf16* orow = p.out + (long long)(tok0 + qrow) * p.ldo + h * kHeadDim + col_t;
+#pragma unroll
+    for (int g = 0; g < 16; ++g)
+      *reinterpret_cast<uint32_t*>(orow + 8 * g) = pack_bf16x2(o[4 * g + 2 * rr] * inv, o[4 * g + 2 * rr + 1] * inv);
   }
 }
 

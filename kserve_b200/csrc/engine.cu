@@ -85,7 +85,7 @@ using namespace b200;
 
 struct b200_engine {
   b200_model_config_t cfg;
-  int num_sms = 148;
+  int num_sms = 132;
   cudaStream_t stream = nullptr;
   cudaStream_t stream2 = nullptr;            // second micro-batch of a tensor-parallel prefill
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -363,8 +363,8 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
       rp.kcache = kc; rp.vcache = vc; rp.page_table = e->d_page_table; rp.max_pages = e->max_pages;
       rp.cos_tab = e->cos_tab; rp.sin_tab = e->sin_tab; rp.nh = e->nh; rp.nkv = e->nkv;
       // RoPE + KV append in the QKV GEMM's epilogue (the separate rope_kv_kernel pass re-read and re-wrote 750 MB per layer
-      // at 0.37 of the HBM peak); B200_NO_ROPE_FUSION=1 / B200_NO_2CTA=1 restore the two-kernel path
-      static const bool rope_fused = getenv("B200_NO_ROPE_FUSION") == nullptr && getenv("B200_NO_2CTA") == nullptr;
+      // at 0.37 of the HBM peak); B200_NO_ROPE_FUSION=1 restores the two-kernel path
+      static const bool rope_fused = getenv("B200_NO_ROPE_FUSION") == nullptr;
       fused_rope = rope_fused;
       GemmArgs a{e->xn + r0 * H, e->cap_T - (int)r0, w.wqkv, e->qkv_cols, T, e->qkv_cols, H, fused_rope ? EPI_ROPE_KV : EPI_STORE, 256, 1,
                  e->qkv + r0 * e->qkv_cols, nullptr, e->qkv_cols, 0, 0, false};
@@ -406,7 +406,7 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
       ap.cu_seqlens = e->d_cu + vw.b0; ap.seq_slot = e->d_seq_slot + vw.b0; ap.nh = e->nh; ap.nkv = e->nkv; ap.scale_log2 = scale_log2;
       static const bool attn_mma = getenv("B200_ATTN_MMA") != nullptr;   // legacy mma.sync kernel for A/B runs
       if (attn_mma) {
-        B200_REQUIRE(kv_off == nullptr, "chunked prefill / prefix reuse needs the tcgen05 attention kernel (unset B200_ATTN_MMA)");
+        B200_REQUIRE(kv_off == nullptr, "chunked prefill / prefix reuse needs the wgmma attention kernel (unset B200_ATTN_MMA)");
         if ((rc = launch_attn_prefill(ap, B, max_len, s))) return rc;
       } else {
         AttnTcParams tp_{};
@@ -655,9 +655,8 @@ static int decode_step_enqueue(b200_engine* e) {
 // that walks the step's weight-streaming GEMMs ahead of the chain (prefetch.cuh).
 template <class Enqueue>
 static int graph_step(b200_engine* e, int key, Enqueue&& enqueue) {
-  // opt-in (B200_PREFETCHER=1): measured r02 (profiles/r02_prefetch_timelines.md) — the head prefetch does not shorten the
-  // step: each GEMM's post-wait time is a latency chain (B tiles -> MMA -> second ring fill -> epilogue), not HBM time,
-  // and the extra requests compete with the kernels that are streaming
+  // opt-in (B200_PREFETCHER=1): each GEMM's post-wait time is a latency chain (B tiles -> MMA -> second ring fill -> epilogue),
+  // not HBM time, so the head prefetch is not expected to shorten the step, and its requests compete with the streaming kernels
   static const bool pf_on = getenv("B200_PREFETCHER") != nullptr;
   auto it = e->graphs.find(key);
   if (it == e->graphs.end()) {
@@ -1226,7 +1225,7 @@ static int copy_cols(bf16* dst, const bf16* src, long long rows, long long src_c
 extern "C" {
 
 const char* b200_last_error(void) { return g_last_error.c_str(); }
-const char* b200_version(void) { return "kserve_b200 0.2 (sm_100a)"; }
+const char* b200_version(void) { return "kserve_b200 0.3 (sm_90a)"; }
 
 int b200_nccl_unique_id(void* out128) {
   Nccl& n = Nccl::get();
@@ -1255,7 +1254,7 @@ int b200_engine_create(const b200_model_config_t* c, const void* nccl_id, b200_e
   B200_CUDA_OK(cudaSetDevice(c->device));
   cudaDeviceProp prop;
   B200_CUDA_OK(cudaGetDeviceProperties(&prop, c->device));
-  B200_REQUIRE(prop.major == 10, std::string("kserve_b200 kernels are built for sm_100a only; device is sm_") +
+  B200_REQUIRE(prop.major == 9 && prop.minor == 0, std::string("kserve_b200 kernels are built for sm_90a only; device is sm_") +
                                      std::to_string(prop.major) + std::to_string(prop.minor));
   std::unique_ptr<b200_engine> e(new b200_engine());
   e->cfg = *c;

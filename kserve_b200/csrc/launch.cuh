@@ -9,8 +9,7 @@
 #include "attention.cuh"
 #include "attention_tc.cuh"
 #include "common.cuh"
-#include "gemm_tcgen05.cuh"
-#include "gemm_2cta.cuh"
+#include "gemm_wgmma.cuh"
 #include "ops.cuh"
 #include "p2p.cuh"
 #include "moe.cuh"
@@ -118,29 +117,6 @@ int launch_gemm_inst(const CUtensorMap* ta, const CUtensorMap* tb, const GemmPar
   return 0;
 }
 
-template <int EPI>
-int launch_gemm_2cta_inst(const CUtensorMap* ta, const CUtensorMap* tb, const GemmParams& p, int num_sms, cudaStream_t s) {
-  auto kern = gemm_tn_2cta_kernel<EPI>;
-  static bool configured = false;
-  if (!configured) {
-    B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, k2SmemBytes));
-    configured = true;
-  }
-  const int units = ((p.m_tiles + 1) / 2) * p.n_tiles;
-  const int clusters = std::min(units, num_sms / 2);
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * clusters); cfg.blockDim = dim3(kGemmThreads); cfg.dynamicSmemBytes = k2SmemBytes; cfg.stream = s;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = (pdl_enabled() && pdl_phase()) ? 2 : 1;
-  B200_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, *ta, *tb, p));
-  return 0;
-}
-
 // Host side of the weight-stream prefetch (prefetch.cuh): while a decode step is being enqueued, every weight-streaming
 // GEMM takes the next index of the step's table; in `recording` mode (first, eager enqueue of a graph key) its
 // descriptor is appended, in capture mode the engine launches the prefetch of the NEXT table entry beside it.
@@ -195,13 +171,7 @@ inline int launch_gemm(TmapCache& cache, const GemmArgs& a, int num_sms, cudaStr
   p.hint_b = a.stream_a ? kEvictLast : kEvictNormal;
   p.m_rt = a.m_rt; p.n_rt = a.n_rt; p.row_off = a.row_off; p.swap_ab = a.stream_a ? 1 : 0;
   p.group_m_tiles = 0; p.group_out_stride = a.group_out_stride;
-  {
-    // r02 (tools/prefill_gemm.py, T = 32768): raster groups of 12 m-pairs + cache-streaming output stores: gate/up 5.47 -> 4.76 ms,
-    // down 3.34 -> 2.57 ms, qkv 1.126 -> 1.108 ms (the 940 MB output stream no longer evicts the A / B tiles other CTAs re-read)
-    static const int gp = getenv("B200_2CTA_GROUP") ? atoi(getenv("B200_2CTA_GROUP")) : 12;
-    static const int cs = getenv("B200_2CTA_CS") ? atoi(getenv("B200_2CTA_CS")) : 1;
-    p.group_pairs = gp; p.stream_out = cs;
-  }
+  p.stream_out = a.stream_a ? 0 : 1;   // prefill outputs are read by a later kernel only: keep them from evicting A / B tiles
   if (a.groups > 0) {
     B200_REQUIRE(a.stream_a && a.n_rt && a.row_off && !a.m_rt && a.N <= a.block_n, "grouped GEMM: swap-AB with per-group n_rt / row_off");
     p.group_m_tiles = p.m_tiles;
@@ -243,25 +213,13 @@ inline int launch_gemm(TmapCache& cache, const GemmArgs& a, int num_sms, cudaStr
   B200_REQUIRE(p.splits == 1 || a.epi == EPI_T_PARTIAL, "split-K only with the fp32 partial epilogue");
   p.rope_tok_seq = nullptr; p.rope_tok_pos = nullptr; p.rope_page_table = nullptr; p.rope_max_pages = 0;
   p.rope_kcache = nullptr; p.rope_vcache = nullptr; p.rope_cos = nullptr; p.rope_sin = nullptr; p.rope_nh = 0; p.rope_nkv = 0;
-  const bool use_2cta = getenv("B200_NO_2CTA") == nullptr;
   if (a.epi == EPI_ROPE_KV) {
-    B200_REQUIRE(use_2cta && a.block_n == 256 && a.rope && a.N == (a.rope->nh + 2 * a.rope->nkv) * kHeadDim,
-                 "EPI_ROPE_KV is the 2-CTA prefill QKV projection");
+    B200_REQUIRE(a.block_n == 256 && a.rope && a.N == (a.rope->nh + 2 * a.rope->nkv) * kHeadDim,
+                 "EPI_ROPE_KV is the prefill QKV projection with 256-column tiles");
     p.rope_tok_seq = a.rope->tok_seq; p.rope_tok_pos = a.rope->tok_pos; p.rope_page_table = a.rope->page_table;
     p.rope_max_pages = a.rope->max_pages; p.rope_kcache = a.rope->kcache; p.rope_vcache = a.rope->vcache;
     p.rope_cos = a.rope->cos_tab; p.rope_sin = a.rope->sin_tab; p.rope_nh = a.rope->nh; p.rope_nkv = a.rope->nkv;
-    const CUtensorMap* tb2;
-    int rc2 = cache.get(a.B, a.b_rows, a.K, 128, &tb2);
-    if (rc2) return rc2;
-    return launch_gemm_2cta_inst<EPI_ROPE_KV>(ta, tb2, p, num_sms, s);
-  }
-  if (use_2cta && a.block_n == 256 && a.epi <= EPI_SWIGLU) {
-    const CUtensorMap* tb2;
-    int rc2 = cache.get(a.B, a.b_rows, a.K, 128, &tb2);   // each CTA of the pair stages half of the 256 weight rows
-    if (rc2) return rc2;
-    if (a.epi == EPI_STORE) return launch_gemm_2cta_inst<EPI_STORE>(ta, tb2, p, num_sms, s);
-    if (a.epi == EPI_STORE_RES) return launch_gemm_2cta_inst<EPI_STORE_RES>(ta, tb2, p, num_sms, s);
-    return launch_gemm_2cta_inst<EPI_SWIGLU>(ta, tb2, p, num_sms, s);
+    return launch_gemm_inst<256, EPI_ROPE_KV>(ta, tb, p, grid, s);
   }
 #define B200_GEMM_CASE(BN, E) \
   if (a.block_n == BN && a.epi == E) return launch_gemm_inst<BN, E>(ta, tb, p, grid, s);
@@ -338,7 +296,7 @@ inline int launch_attn_prefill(const AttnPrefillParams& p, int B, int max_len, c
   return 0;
 }
 
-// tcgen05 prefill attention: q rows [q_rows][ldq] (head h at column h*128), paged caches [num_pages][nkv][64][128]
+// wgmma prefill attention: q rows [q_rows][ldq] (head h at column h*128), paged caches [num_pages][nkv][64][128]
 inline int launch_attn_prefill_tc(TmapCache& cache, const bf16* q, int q_rows, long long ldq, const bf16* kcache,
                                   const bf16* vcache, int num_pages, const AttnTcParams& p, int B, int max_len, cudaStream_t s) {
   static bool configured = false;

@@ -1,7 +1,7 @@
 // Sparse mixture-of-experts block (Mixtral: SURVEY.md §8a row 18, transformers modeling_mixtral.py:62-135):
 //   router  : logits = xn * Wr^T (bf16 result), softmax in fp32, top-k (k = 2), renormalised fp32 weights
 //   dispatch: tokens are grouped per expert into one compact row buffer (deterministic order: token index)
-//   experts : the same tcgen05 GEMM kernels as the dense MLP, one launch per expert, bounded at run time by the
+//   experts : the same wgmma GEMM kernels as the dense MLP, one launch per expert, bounded at run time by the
 //             device-side token count of that expert (GemmParams::m_rt / n_rt / row_off)
 //   combine : out[t] = bf16(bf16(y_e1[t] * w1) + bf16(y_e2[t] * w2)) in ascending expert order, exactly the
 //             bf16 index_add_ sequence of MixtralExperts.forward, then residual add + next RMSNorm (fused)

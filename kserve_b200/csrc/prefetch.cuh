@@ -6,15 +6,11 @@
 // bytes, i.e. pure latency.  The weights, however, depend on nothing.  While GEMM g of the step runs, a tiny kernel on a
 // forked branch of the step's CUDA graph issues `cp.async.bulk.prefetch.tensor.2d.L2` for the HEAD of GEMM g+1's weight
 // stream: for every CTA of that launch, the first `cap_kb` k-block tiles of exactly the work list (gemm_get_seg) the CTA
-// will walk.  The 126 MB L2 is the staging buffer: HBM keeps streaming through the stalls of the chain and the next
+// will walk.  The L2 (50 MB on H100) is the staging buffer: HBM keeps streaming through the stalls of the chain and the next
 // GEMM finds the start of its stream in L2.  The kernel only issues prefetches and exits (no spinning, no residency).
 //
-// (A first version kept one prefetch CTA resident per SM for the whole step, paced by progress counters the GEMM CTAs
-// published: the resident CTAs pinned 32 SMs to the shared-memory carve-out of the first small kernel that reached them
-// — the 165 KB GEMM CTAs could never become resident there — and an atomicMax per k-block cost the TMA producer thread
-// a third of its issue rate; r02 timelines in profiles/.)
 #pragma once
-#include "gemm_tcgen05.cuh"
+#include "gemm_wgmma.cuh"
 
 namespace b200 {
 

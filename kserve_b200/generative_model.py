@@ -152,7 +152,7 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
         cfg = self.model_config
         arch = (cfg.get("architectures") or ["LlamaForCausalLM"])[0]
         if not arch.endswith("ForCausalLM") or cfg.get("model_type", "llama") not in ("llama", "mistral", "mixtral"):
-            raise OpenAIError(f"architecture {arch} is not supported by the B200 runtime (Llama / Mistral / Mixtral decoders only)")
+            raise OpenAIError(f"architecture {arch} is not supported by the H100 runtime (Llama / Mistral / Mixtral decoders only)")
         if self._tokenizer is None and self.model_id_or_path and os.path.exists(
                 os.path.join(self.model_id_or_path, "tokenizer.json")):
             from transformers import AutoTokenizer
@@ -178,15 +178,15 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
             # inside the window sliding-window attention IS full attention, so serving at most `window` tokens is exact
             if self._user_max_len is not None:
                 raise OpenAIError(f"max_model_len ({self.max_length}) exceeds the checkpoint's sliding_window ({window}); "
-                                  "the B200 runtime implements full attention only")
+                                  "the H100 runtime implements full attention only")
             logger.warning("sliding_window=%d < max length %d: serving at most %d tokens (full attention == sliding "
                            "window inside the window)", window, self.max_length, window)
             self.max_length = int(window)
         for key in ("attention_bias", "mlp_bias"):
             if cfg.get(key):
-                raise OpenAIError(f"config.{key}=true is not supported by the B200 runtime")
+                raise OpenAIError(f"config.{key}=true is not supported by the H100 runtime")
         if cfg.get("hidden_act", "silu") != "silu":
-            raise OpenAIError(f"hidden_act={cfg.get('hidden_act')} is not supported by the B200 runtime (silu only)")
+            raise OpenAIError(f"hidden_act={cfg.get('hidden_act')} is not supported by the H100 runtime (silu only)")
         # checkpoint generation defaults: transformers merges the None fields of the request's GenerationConfig from
         # model.generation_config (generation/utils.py:1693-1701) — this is how instruct checkpoints turn sampling on (q9)
         self.generation_defaults = dict(self._generation_defaults or {})
@@ -198,7 +198,7 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
         if ck_dtype not in (None, "bfloat16"):
             # the reference's `--dtype auto` would compute in the checkpoint's type (__main__.py:249-259); this runtime's
             # only arithmetic type is bfloat16 (fp32 accumulation), so other checkpoints are converted at load
-            logger.warning("checkpoint dtype %s: weights are converted to bfloat16, the only compute type of the B200 runtime",
+            logger.warning("checkpoint dtype %s: weights are converted to bfloat16, the only compute type of the H100 runtime",
                            ck_dtype)
         eos = cfg.get("eos_token_id")
         self.eos_token_ids = [] if eos is None else ([int(e) for e in eos] if isinstance(eos, list) else [int(eos)])

@@ -21,7 +21,7 @@ def create_application(dataplane: OpenAIDataPlane, batcher: Optional[Tuple[int, 
     server; pkg/batcher/handler.go:222-266 ServeHTTP).  Concurrent `:predict` requests are merged into ONE downstream
     predict whose instances are the concatenation of theirs; every caller gets `{"message", "batchId", "predictions"}`
     with its own slice."""
-    app = FastAPI(title="KServe ModelServer (B200 runtime)", version=dataplane._server_version)
+    app = FastAPI(title="KServe ModelServer (H100 runtime)", version=dataplane._server_version)
     dp: DataPlane = dataplane
     batch_handler = None
     if batcher is not None:

@@ -110,10 +110,10 @@ def rope_inv_freq(cfg: Dict[str, Any], head_dim: int) -> torch.Tensor:
     rp = rope_parameters(cfg)
     kind = rp["rope_type"]
     if kind not in SUPPORTED_ROPE_TYPES:
-        raise ValueError(f"rope_scaling type '{kind}' is not supported by the B200 runtime (supported: "
+        raise ValueError(f"rope_scaling type '{kind}' is not supported by the H100 runtime (supported: "
                          f"{', '.join(SUPPORTED_ROPE_TYPES)}); refusing to load a model that would generate wrong tokens")
     if float(rp.get("partial_rotary_factor", cfg.get("partial_rotary_factor", 1.0)) or 1.0) != 1.0:
-        raise ValueError("partial_rotary_factor != 1 is not supported by the B200 runtime")
+        raise ValueError("partial_rotary_factor != 1 is not supported by the H100 runtime")
     base = float(rp["rope_theta"])
     inv_freq = 1.0 / (base ** (torch.arange(0, head_dim, 2, dtype=torch.int64).to(torch.float) / head_dim))
     if kind == "linear":

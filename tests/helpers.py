@@ -37,6 +37,12 @@ def load_case(name):
                 topk_vals=torch.from_numpy(z["topk_vals"]), topk_idx=torch.from_numpy(z["topk_idx"]))
     if "step_logits" in z:
         case["step_logits"] = torch.from_numpy(z["step_logits"])  # [B, T, V]
+    if "step_logits_bf16" in z:   # the same logits (bf16 values) as 16-bit patterns, rows split over <name>.npz and <name>.2.npz
+        parts = [z["step_logits_bf16"]]
+        more = os.path.join(GOLDEN, name + ".2.npz")
+        if os.path.exists(more):
+            parts.append(np.load(more)["step_logits_bf16"])
+        case["step_logits"] = torch.from_numpy(np.concatenate(parts)).view(torch.bfloat16).float()
     if "step0_logits" in z:
         case["step0_logits"] = torch.from_numpy(z["step0_logits"].astype(np.float32))
     if "sub_logits" in z:     # big-vocabulary cases: every step's logits on a fixed subset of the columns, [B, T, n]

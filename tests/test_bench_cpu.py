@@ -12,21 +12,12 @@ def test_algorithmic_work_matches_the_survey_figures():
     assert abs(a["layer_params"] - 218_112_000) <= 2 * 4096                # the survey also counts the two norm vectors
     assert abs(a["weight_bytes"] - 15.01e9) < 0.01e9                    # 32 layers + lm_head, bf16
     assert a["kv_bytes_per_token"] == 131_072
-    assert abs(a["decode_bytes_per_step"] - 19.57e9) < 0.01e9          # -> 2.98 ms at 6577 GB/s
+    assert abs(a["decode_bytes_per_step"] - 19.57e9) < 0.01e9          # -> 5.84 ms at 3.35 TB/s
     assert abs(a["prefill_flops"] - 466e12) < 1e12                      # 457.4 GEMM + 8.8 causal attention + lm_head
     half = bench.algorithmic(bench.LLAMA3_8B, 32, 1024, 128, tp=2)
     assert abs(half["decode_bytes_per_step"] * 2 - a["decode_bytes_per_step"]) < 1 and abs(half["prefill_flops"] * 2 - a["prefill_flops"]) < 1
     m = bench.algorithmic(bench.MIXTRAL_8X7B, 32, 1024, 128, tp=4)
     assert abs(m["weight_bytes"] * 4 - 93.4e9) < 0.5e9                  # all 8 experts stream (46.7 B params incl. the embedding)
-
-
-def test_traffic_comes_from_the_committed_capture_only_on_its_configuration():
-    t = bench.ncu_decode_traffic(bench.LLAMA3_8B, 32, 1024, 128, 1)
-    a = bench.algorithmic(bench.LLAMA3_8B, 32, 1024, 128)["decode_bytes_per_step"]
-    assert t is not None and 1.0 <= t / a < 1.1                         # no wasted re-reads
-    assert bench.ncu_decode_traffic(bench.LLAMA3_8B, 64, 1024, 128, 1) is None
-    assert bench.ncu_decode_traffic(bench.LLAMA3_8B, 32, 1024, 128, 2) is None
-    assert bench.ncu_decode_traffic(bench.MIXTRAL_8X7B, 32, 1024, 128, 1) is None
 
 
 def test_cpu_thread_policy_and_peaks():

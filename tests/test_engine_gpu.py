@@ -20,11 +20,12 @@ STATS = {}
 
 
 def _record(name, **kw):
+    """Parity statistics of the run; written as JSON to the file KSERVE_PARITY_STATS names, if set."""
     STATS[name] = kw
-    out = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
-    os.makedirs(out, exist_ok=True)
-    with open(os.path.join(out, "parity_stats.json"), "w") as f:
-        json.dump(STATS, f, indent=1)
+    path = os.environ.get("KSERVE_PARITY_STATS")
+    if path:
+        with open(path, "w") as f:
+            json.dump(STATS, f, indent=1)
 
 
 CASES = ["tiny_g2_ids", "tiny_g2_text", "tiny_g2_padinfer", "tiny_g4_ids", "tiny_g4_b1",
@@ -171,7 +172,7 @@ def headline_engines():
 @pytest.mark.parametrize("name", HEADLINE)
 def test_headline_shapes_1024_prompt_tokens(headline_engines, name):
     """VERDICT r01 weak #1: the headline configuration's shapes against the oracle — S = 1024 (16 KV tiles through
-    attn_prefill_tc_kernel, 4096 packed rows through the 2-CTA prefill GEMMs), decode at context 1025..1040, a ragged
+    attn_prefill_tc_kernel, 4096 packed rows through the 256-column prefill GEMMs), decode at context 1025..1040, a ragged
     U[512,1024] left-padded batch, V = 128256.  Teacher-forced: every step's logits on 4096 fixed columns + the oracle's
     top-16; peaked cases additionally require the free-running greedy ids to be the oracle's, token for token."""
     c = load_case(name)

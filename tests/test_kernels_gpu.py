@@ -1,4 +1,4 @@
-"""Single-kernel parity: each sm_100a kernel, called through the C ABI on device pointers, against a
+"""Single-kernel parity: each sm_90a kernel, called through the C ABI on device pointers, against a
 plain PyTorch fp32 statement of the same op (floating-point kernels keep a torch reference; tolerances
 are written next to each check)."""
 import ctypes as C
@@ -251,7 +251,7 @@ def test_attn_prefill(lib, nh, nkv, lens):
 @pytest.mark.parametrize("nh,nkv", [(4, 2), (8, 2), (32, 8)])
 @pytest.mark.parametrize("lens", [[5], [64, 1, 130], [200, 63, 65, 128, 129], [700, 257]])
 def test_attn_prefill_tcgen05(lib, nh, nkv, lens):
-    """The tcgen05 / TMEM prefill attention (engine default) against the fp32 statement of causal GQA attention."""
+    """The wgmma prefill attention (engine default) against the fp32 statement of causal GQA attention."""
     B = len(lens)
     kc, vc, pt, max_pages, kd, vd = _build_cache(B, lens, nkv, seed=21)
     T = sum(lens)

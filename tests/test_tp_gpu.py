@@ -1,8 +1,7 @@
 """Tensor parallel on real GPUs: TP = 2 / 4 / 8 engines (peer-memory all-reduce per row-parallel GEMM, vocab-parallel
 LM head) against the oracle fixtures — teacher-forced logits within the stated tolerance, greedy ids by the margin rule,
 and exactly on the peaked fixture.  The 8-KV-head fixtures shard down to one KV head per GPU at TP = 8 (the SCALE run's
-shape).  Skipped when the box has fewer GPUs than the degree (the driver's GPUTEST box has one; run with
-`gpurun --gpus 8 -- python -m pytest tests/test_tp_gpu.py -m gpu`)."""
+shape).  Skipped on a machine with fewer GPUs than the degree."""
 import json
 import os
 import subprocess

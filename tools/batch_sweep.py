@@ -1,4 +1,4 @@
-"""BASELINE.json configs[1]: Llama-3-8B bf16 on 1xB200, batch sweep 1-64, 1024-in/128-out.  One engine, every batch
+"""BASELINE.json configs[1]: Llama-3-8B bf16 on 1xH100, batch sweep 1-64, 1024-in/128-out.  One engine, every batch
 size timed like bench.py (device-resident prompt, CUDA events on the engine stream) plus the end-to-end call."""
 import json
 import os
@@ -46,7 +46,7 @@ def main():
         print(json.dumps(rows[-1]), flush=True)
     out = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out", "batch_sweep.json")
     os.makedirs(os.path.dirname(out), exist_ok=True)
-    json.dump(dict(workload="Llama-3-8B bf16 random-init, 1024-in/128-out, greedy, 1xB200", peaks=peaks, rows=rows), open(out, "w"), indent=1)
+    json.dump(dict(workload="Llama-3-8B bf16 random-init, 1024-in/128-out, greedy, 1xH100", peaks=peaks, rows=rows), open(out, "w"), indent=1)
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""BASELINE.json configs[4]: batcher maxBatchSize=64 maxLatency=50ms fronting Llama-3-8B on 1xB200, 512 concurrent
+"""BASELINE.json configs[4]: batcher maxBatchSize=64 maxLatency=50ms fronting Llama-3-8B on 1xH100, 512 concurrent
 closed-loop clients, one instance (one ragged token-id prompt, U[512,1024] tokens) per request.
 
 The Go sidecar cannot be built here (no Go toolchain): the same trigger state machine (C ABI b200_batcher_*) is

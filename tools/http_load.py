@@ -1,5 +1,5 @@
 """BASELINE.json configs[4] over HTTP: 512 concurrent closed-loop clients against the real model server (uvicorn +
-FastAPI routes of kserve_b200.kserve_api) fronting Llama-3-8B dims (random init) on one B200.
+FastAPI routes of kserve_b200.kserve_api) fronting Llama-3-8B dims (random init) on one H100.
 
     MODE=continuous  POST /openai/v1/completions (token-id prompts) served by the iteration-level scheduler
                      (--continuous_batching, chunked prefill, up to SLOTS resident sequences)
