@@ -205,6 +205,18 @@ __device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* map, int c
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
+// 2D tile store shared -> global (elements outside the map's extents are not written), tracked by bulk groups.
+// Generic-proxy writes of the source tile must be made visible with fence_proxy_async_shared() before the issue.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* smem_src, int c_inner, int c_outer,
+                                             uint64_t hint) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3}], [%1], %4;"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(smem_src)), "r"(c_inner), "r"(c_outer), "l"(hint)
+               : "memory");
+}
+__device__ __forceinline__ void fence_proxy_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }  // sources reusable
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------
 // wgmma (sm_90a warpgroup MMA): all 128 threads of a warpgroup issue it together; the fp32 accumulator of an

@@ -5,12 +5,11 @@
 //                    registers); the accumulators are staged through shared memory so that the fused epilogue sees
 //                    one tile row per thread, 32 consecutive columns at a time
 //
-// The same kernel serves both phases of the LLM path (SURVEY.md §8a rows 13-17):
-//   * prefill  : A = activations [T,K], B = weight [N_out,K]           -> row-major epilogues
-//   * decode   : A = weight [N_out,K] (M = N_out), B = activations [batch,K] ("swap-AB": the 128-row MMA
-//                M dimension is filled by weight rows, the small batch rides in the MMA N dimension, so no
-//                tensor-core work is wasted on padding and each CTA streams a contiguous weight slab)
-//                -> transposed epilogues, optional split-K with fp32 partials.
+// This file holds the decode kernel (SURVEY.md §8a rows 13-17): A = weight [N_out,K] (M = N_out), B = activations
+// [batch,K] ("swap-AB": the 128-row MMA M dimension is filled by weight rows, the small batch rides in the MMA N
+// dimension, so no tensor-core work is wasted on padding and each CTA streams a contiguous weight slab) -> transposed
+// epilogues, optional split-K with fp32 partials.  The prefill GEMMs (A = activations [T,K], B = weight [N_out,K],
+// row-major epilogues) run gemm_prefill_kernel (gemm_prefill.cuh), which shares the parameters and the schedule.
 #pragma once
 #include "common.cuh"
 
@@ -65,6 +64,7 @@ struct GemmParams {
   const bf16* rope_cos; const bf16* rope_sin;                // [max_pos][64]
   int rope_nh, rope_nkv;
   int stream_out;          // row-major epilogues: cache-streaming output stores
+  int out_tma;             // row-major epilogues: `out` is addressable by TMA (16-byte aligned base and row pitch)
   int sched;
   int sk_slots;            // partial slots per tile
   float* sk_ws;            // [m_tiles][sk_slots][BLOCK_N][128] fp32
@@ -79,12 +79,13 @@ constexpr int kStgStride = 132;   // floats between two staged accumulator colum
 
 template <int BLOCK_N>
 struct GemmCfg {
+  static_assert(BLOCK_N <= 64, "swap-AB tiles carry the batch in N");
   static constexpr int kABytes = kGemmBlockM * kGemmBlockK * 2;  // 16 KB
   static constexpr int kBBytes = BLOCK_N * kGemmBlockK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = (BLOCK_N >= 256) ? 3 : 8;
+  static constexpr int kStages = 8;
   static constexpr int kChunk = (BLOCK_N >= 32) ? 32 : 16;             // columns one epilogue thread takes at a time
-  static constexpr int kRoundCols = (BLOCK_N < 128) ? BLOCK_N : 128;   // columns staged per epilogue round (one head)
+  static constexpr int kRoundCols = BLOCK_N;                           // columns staged per epilogue round
   static constexpr int kChunks = kRoundCols / kChunk;
   static constexpr int kStgBytes = kRoundCols * kStgStride * 4;
   static constexpr int kSmemBytes = kStages * kStageBytes + kStgBytes + 1024 /*align slack*/ + 256 /*barriers*/;
@@ -182,6 +183,7 @@ template <int BLOCK_N, int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const GemmParams p) {
+  static_assert(EPI == EPI_T_STORE || EPI == EPI_T_SWIGLU || EPI == EPI_T_PARTIAL, "swap-AB epilogues only");
   TraceScope _ts(TK_GEMM + 100 * EPI + 1000 * (p.M >> 7));
   using Cfg = GemmCfg<BLOCK_N>;
   constexpr int STAGES = Cfg::kStages;
@@ -343,61 +345,6 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           s0[kStgStride + 8] = accum[4 * j + 3];
         }
         consumer_bar();
-        if constexpr (EPI == EPI_ROPE_KV) {
-          // the round's 128 columns are one whole head; this warpgroup takes dims [32 * half, 32 * half + 32) and their
-          // rotate-half partners 64 further (V: the same two 32-column chunks)
-          const int col0 = n0 + r0;
-          const int head = col0 >> 7;
-          if (m < M_rt) {
-            const int pos = p.rope_tok_pos[m + roff_a];
-            const int page = p.rope_page_table[(long long)p.rope_tok_seq[m + roff_a] * p.rope_max_pages + (pos >> 6)];
-            const long long page_row = (long long)page * p.rope_nkv * 64 + (pos & 63);   // row of kv head 0 in [..][64][128]
-            const int c = 32 * half;
-            if (head >= p.rope_nh + p.rope_nkv) {           // ---- V head: copy to the cache
-              bf16* vrow = p.rope_vcache + (page_row + (long long)(head - p.rope_nh - p.rope_nkv) * 64) * 128;
-#pragma unroll
-              for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-                for (int j = 0; j < 32; j += 8) {
-                  const float* sv = stg + (hh * 64 + c + j) * kStgStride + t;
-                  uint4 o;
-                  o.x = pack_bf16x2(sv[0], sv[kStgStride]);
-                  o.y = pack_bf16x2(sv[2 * kStgStride], sv[3 * kStgStride]);
-                  o.z = pack_bf16x2(sv[4 * kStgStride], sv[5 * kStgStride]);
-                  o.w = pack_bf16x2(sv[6 * kStgStride], sv[7 * kStgStride]);
-                  *reinterpret_cast<uint4*>(vrow + hh * 64 + c + j) = o;
-                }
-            } else {                                         // ---- q or k head: rotate-half RoPE on the pairs (d, d + 64)
-              bf16* dst = head < p.rope_nh ? reinterpret_cast<bf16*>(p.out) + (long long)(m + roff_a) * p.ldo + col0
-                                           : p.rope_kcache + (page_row + (long long)(head - p.rope_nh) * 64) * 128;
-#pragma unroll
-              for (int j = 0; j < 32; j += 8) {
-                const uint4 cu = *reinterpret_cast<const uint4*>(p.rope_cos + (long long)pos * 64 + c + j);
-                const uint4 su = *reinterpret_cast<const uint4*>(p.rope_sin + (long long)pos * 64 + c + j);
-                const uint32_t cw[4] = {cu.x, cu.y, cu.z, cu.w}, sw[4] = {su.x, su.y, su.z, su.w};
-                const float* s1 = stg + (c + j) * kStgStride + t;
-                const float* s2 = s1 + 64 * kStgStride;
-                float o1[8], o2[8];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                  const float2 cs = unpack_bf16x2(cw[u]), sn = unpack_bf16x2(sw[u]);
-                  const float a0 = bf16_round(s1[(2 * u) * kStgStride]), a1 = bf16_round(s1[(2 * u + 1) * kStgStride]);
-                  const float b0 = bf16_round(s2[(2 * u) * kStgStride]), b1 = bf16_round(s2[(2 * u + 1) * kStgStride]);
-                  o1[2 * u] = bf16_round(a0 * cs.x) + bf16_round(-b0 * sn.x);
-                  o1[2 * u + 1] = bf16_round(a1 * cs.y) + bf16_round(-b1 * sn.y);
-                  o2[2 * u] = bf16_round(b0 * cs.x) + bf16_round(a0 * sn.x);
-                  o2[2 * u + 1] = bf16_round(b1 * cs.y) + bf16_round(a1 * sn.y);
-                }
-                uint4 w1, w2;
-                w1.x = pack_bf16x2(o1[0], o1[1]); w1.y = pack_bf16x2(o1[2], o1[3]); w1.z = pack_bf16x2(o1[4], o1[5]); w1.w = pack_bf16x2(o1[6], o1[7]);
-                w2.x = pack_bf16x2(o2[0], o2[1]); w2.y = pack_bf16x2(o2[2], o2[3]); w2.z = pack_bf16x2(o2[4], o2[5]); w2.w = pack_bf16x2(o2[6], o2[7]);
-                *reinterpret_cast<uint4*>(dst + c + j) = w1;
-                *reinterpret_cast<uint4*>(dst + 64 + c + j) = w2;
-              }
-            }
-          }
-          continue;
-        }
         // this warpgroup's chunks of the round: half, half + 2
 #pragma unroll
         for (int ch = half; ch < Cfg::kChunks; ch += 2) {
@@ -425,68 +372,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
 #pragma unroll
             for (int j = 0; j < CH; ++j) v[j] += acc[j];
           }
-          if constexpr (EPI == EPI_STORE || EPI == EPI_STORE_RES) {
-            if (m < M_rt) {
-              bf16* orow = reinterpret_cast<bf16*>(p.out) + (long long)(m + roff_a) * p.ldo + n0 + c0;
-              const bf16* rrow = (EPI == EPI_STORE_RES) ? p.residual + (long long)(m + roff_a) * p.ldo + n0 + c0 : nullptr;
-              const bool vec = (nvalid == CH) && ((p.ldo & 7) == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 15) == 0);
-              if (vec) {
-#pragma unroll
-                for (int j = 0; j < CH; j += 8) {
-                  float f[8];
-#pragma unroll
-                  for (int u = 0; u < 8; ++u) f[u] = v[j + u];
-                  if constexpr (EPI == EPI_STORE_RES) {
-                    uint4 rr = *reinterpret_cast<const uint4*>(rrow + j);
-                    const uint32_t rw[4] = {rr.x, rr.y, rr.z, rr.w};
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                      float2 r2 = unpack_bf16x2(rw[u]);
-                      f[2 * u] = bf16_round(f[2 * u]) + r2.x;
-                      f[2 * u + 1] = bf16_round(f[2 * u + 1]) + r2.y;
-                    }
-                  }
-                  uint4 o;
-                  o.x = pack_bf16x2(f[0], f[1]);
-                  o.y = pack_bf16x2(f[2], f[3]);
-                  o.z = pack_bf16x2(f[4], f[5]);
-                  o.w = pack_bf16x2(f[6], f[7]);
-                  st_out_v4(orow + j, o, p.stream_out);
-                }
-              } else {
-                for (int j = 0; j < nvalid; ++j) {
-                  float f = v[j];
-                  if constexpr (EPI == EPI_STORE_RES) f = bf16_round(f) + __bfloat162float(rrow[j]);
-                  orow[j] = __float2bfloat16_rn(f);
-                }
-              }
-            }
-          } else if constexpr (EPI == EPI_SWIGLU) {
-            // columns [c0, c0+16) = gate, [c0+16, c0+32) = up of output columns (n0+c0)/2 + j
-            static_assert(EPI != EPI_SWIGLU || CH == 32, "SWIGLU needs 32-column chunks");
-            if (m < M_rt) {
-              const int oc = (n0 + c0) >> 1;
-              bf16* orow = reinterpret_cast<bf16*>(p.out) + (long long)(m + roff_a) * p.ldo + oc;
-              float h[16];
-#pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                const float g = bf16_round(v[j]);
-                const float up = bf16_round(v[16 + j]);
-                h[j] = bf16_round(silu_f(g)) * up;
-              }
-              if (oc + 16 <= p.out_cols && (p.ldo & 7) == 0) {
-                uint4 o0, o1;
-                o0.x = pack_bf16x2(h[0], h[1]);   o0.y = pack_bf16x2(h[2], h[3]);
-                o0.z = pack_bf16x2(h[4], h[5]);   o0.w = pack_bf16x2(h[6], h[7]);
-                o1.x = pack_bf16x2(h[8], h[9]);   o1.y = pack_bf16x2(h[10], h[11]);
-                o1.z = pack_bf16x2(h[12], h[13]); o1.w = pack_bf16x2(h[14], h[15]);
-                st_out_v4(orow, o0, p.stream_out);
-                st_out_v4(orow + 8, o1, p.stream_out);
-              } else {
-                for (int j = 0; j < 16 && oc + j < p.out_cols; ++j) orow[j] = __float2bfloat16_rn(h[j]);
-              }
-            }
-          } else if constexpr (EPI == EPI_T_STORE) {
+          if constexpr (EPI == EPI_T_STORE) {
             if (m < M_rt) {
               bf16* o = reinterpret_cast<bf16*>(p.out) + out_off + (long long)(n0 + c0 + roff_b) * p.ldo + m;
 #pragma unroll

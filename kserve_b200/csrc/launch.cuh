@@ -9,6 +9,7 @@
 #include "attention.cuh"
 #include "attention_tc.cuh"
 #include "common.cuh"
+#include "gemm_prefill.cuh"
 #include "gemm_wgmma.cuh"
 #include "ops.cuh"
 #include "p2p.cuh"
@@ -59,13 +60,15 @@ inline int make_tmap_2d(CUtensorMap* map, const void* ptr, uint64_t rows, uint64
 }
 
 struct TmapCache {
-  std::map<std::tuple<const void*, uint64_t, uint64_t, uint32_t>, CUtensorMap> maps;
-  int get(const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows, const CUtensorMap** out) {
-    auto key = std::make_tuple(ptr, rows, cols, box_rows);
+  std::map<std::tuple<const void*, uint64_t, uint64_t, uint32_t, uint64_t>, CUtensorMap> maps;
+  // ld_elems: row pitch in elements, 0 = dense rows (cols)
+  int get(const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows, const CUtensorMap** out, uint64_t ld_elems = 0) {
+    if (ld_elems == 0) ld_elems = cols;
+    auto key = std::make_tuple(ptr, rows, cols, box_rows, ld_elems);
     auto it = maps.find(key);
     if (it == maps.end()) {
       CUtensorMap m;
-      int rc = make_tmap_2d(&m, ptr, rows, cols, cols, box_rows);
+      int rc = make_tmap_2d(&m, ptr, rows, cols, ld_elems, box_rows);
       if (rc) return rc;
       it = maps.emplace(key, m).first;
     }
@@ -103,6 +106,19 @@ inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_
   cfg.attrs = attr;
   cfg.numAttrs = (pdl_enabled() && pdl_phase()) ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
+}
+
+template <int EPI>
+int launch_prefill_inst(const CUtensorMap* ta, const CUtensorMap* tb, const CUtensorMap* to, const GemmParams& p, int grid,
+                        cudaStream_t s) {
+  auto kern = gemm_prefill_kernel<EPI>;
+  static bool configured = false;  // per instantiation
+  if (!configured) {
+    B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PrefillCfg<EPI>::kSmemBytes));
+    configured = true;
+  }
+  B200_CUDA_OK(launch_k(kern, dim3(grid), dim3(kGemmThreads), PrefillCfg<EPI>::kSmemBytes, s, *ta, *tb, *to, p));
+  return 0;
 }
 
 template <int BLOCK_N, int EPI>
@@ -219,13 +235,27 @@ inline int launch_gemm(TmapCache& cache, const GemmArgs& a, int num_sms, cudaStr
     p.rope_tok_seq = a.rope->tok_seq; p.rope_tok_pos = a.rope->tok_pos; p.rope_page_table = a.rope->page_table;
     p.rope_max_pages = a.rope->max_pages; p.rope_kcache = a.rope->kcache; p.rope_vcache = a.rope->vcache;
     p.rope_cos = a.rope->cos_tab; p.rope_sin = a.rope->sin_tab; p.rope_nh = a.rope->nh; p.rope_nkv = a.rope->nkv;
-    return launch_gemm_inst<256, EPI_ROPE_KV>(ta, tb, p, grid, s);
+  }
+  p.out_tma = 0;
+  if (a.epi == EPI_STORE || a.epi == EPI_STORE_RES || a.epi == EPI_SWIGLU || a.epi == EPI_ROPE_KV) {
+    B200_REQUIRE(a.block_n == 256 && !a.stream_a && a.groups == 0 && !a.n_rt, "prefill GEMMs use 256-column row-major tiles");
+    // The output map covers exactly the rows a launch may write: M when it is known here, else (device-side m_rt /
+    // row_off) the rows of the activation buffer, whose row index the output rows share.  The kernel hands TMA whole
+    // tiles below the runtime M only; a partial last tile is stored per thread.
+    const CUtensorMap* to = ta;   // (unused placeholder when out_tma == 0)
+    const uint64_t out_rows = (a.m_rt || a.row_off) ? (uint64_t)a.a_rows : (uint64_t)a.M;
+    const uint64_t out_cols = a.epi == EPI_SWIGLU ? (uint64_t)a.out_cols : (uint64_t)a.N;
+    if ((reinterpret_cast<uintptr_t>(a.out) & 15) == 0 && (a.ldo & 7) == 0 && out_cols > 0) {
+      if ((rc = cache.get(a.out, out_rows, out_cols, kGemmBlockM, &to, (uint64_t)a.ldo))) return rc;
+      p.out_tma = 1;
+    }
+    if (a.epi == EPI_STORE) return launch_prefill_inst<EPI_STORE>(ta, tb, to, p, grid, s);
+    if (a.epi == EPI_STORE_RES) return launch_prefill_inst<EPI_STORE_RES>(ta, tb, to, p, grid, s);
+    if (a.epi == EPI_SWIGLU) return launch_prefill_inst<EPI_SWIGLU>(ta, tb, to, p, grid, s);
+    return launch_prefill_inst<EPI_ROPE_KV>(ta, tb, to, p, grid, s);
   }
 #define B200_GEMM_CASE(BN, E) \
   if (a.block_n == BN && a.epi == E) return launch_gemm_inst<BN, E>(ta, tb, p, grid, s);
-  B200_GEMM_CASE(256, EPI_STORE)
-  B200_GEMM_CASE(256, EPI_STORE_RES)
-  B200_GEMM_CASE(256, EPI_SWIGLU)
   B200_GEMM_CASE(16, EPI_T_STORE)
   B200_GEMM_CASE(16, EPI_T_SWIGLU)
   B200_GEMM_CASE(16, EPI_T_PARTIAL)
