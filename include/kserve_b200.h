@@ -64,8 +64,11 @@ int b200_engine_ipc_import(b200_engine_t* e, const void* handles, int32_t n);
  * generative_model.py:249-254).  `data` is the FULL (unsharded) bf16 tensor, row-major, on the host
  * (on_device=0) or on this engine's GPU (on_device=1); the engine copies the shard of its tp_rank and
  * fuses q/k/v and gate/up.  MoE checkpoints use the fused-expert names `mlp.gate.weight` [E,H],
- * `mlp.experts.gate_up_proj` [E,2I,H] and `mlp.experts.down_proj` [E,H,I].  b200_engine_finalize_weights fails if
- * a tensor is missing. */
+ * `mlp.experts.gate_up_proj` [E,2I,H] and `mlp.experts.down_proj` [E,H,I].  Qwen2 checkpoints add the 1-D
+ * projection biases `self_attn.q_proj.bias` [num_heads*128] and `self_attn.{k,v}_proj.bias` [num_kv_heads*128]; they are
+ * sharded like the weights' rows and added in fp32 before the projection's one bf16 rounding (before RoPE).
+ * b200_engine_finalize_weights fails if a tensor is missing: it takes 3 + 9 L tensors, or 3 + 12 L when every layer has
+ * all three biases. */
 int b200_engine_set_weight(b200_engine_t* e, const char* hf_name, const void* data, int on_device,
                            int ndim, const int64_t* shape);
 int b200_engine_finalize_weights(b200_engine_t* e);
@@ -170,6 +173,10 @@ int b200_batcher_tick(b200_batcher_t* b, int64_t now_us, int32_t cap, int64_t* t
  * 5 transposed fp32 split-K partials.  block_n: 256 for epi 0-2, 16/32/64 for epi 3-5. */
 int b200_op_gemm(const void* A, const void* B, void* out, const void* residual, int M, int N, int K, int epi,
                  int block_n, int splits, int64_t ldo, void* stream);
+/* b200_op_gemm with a bf16 bias per output feature, added to the fp32 accumulator before the one bf16 rounding:
+ * epi 0 (block_n 256) adds bias[n] to out[m][n], epi 3 (block_n 16/32/64) adds bias[m] to out[n][m]. */
+int b200_op_gemm_bias(const void* A, const void* B, void* out, const void* residual, int M, int N, int K, int epi,
+                      int block_n, int splits, int64_t ldo, const void* bias, void* stream);
 int b200_op_rmsnorm(void* x, const void* w, void* xn, int rows, int H, float eps, const float* partial,
                     int splits, const void* y, void* stream);
 int b200_op_attn_prefill(const void* q, int64_t ldq, void* out, int64_t ldo, const void* kcache,

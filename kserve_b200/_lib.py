@@ -66,6 +66,7 @@ def load() -> C.CDLL:
     lib.b200_run_staged_timed.argtypes = [vp, i32, C.POINTER(C.c_float), C.POINTER(C.c_float)]
     lib.b200_fetch_staged.argtypes = [vp, vp, C.POINTER(i32), C.POINTER(i32)]
     lib.b200_op_gemm.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, i64, vp]
+    lib.b200_op_gemm_bias.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, i64, vp, vp]
     lib.b200_op_rmsnorm.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_float, vp, C.c_int, vp, vp]
     lib.b200_op_attn_prefill.argtypes = [vp, i64, vp, i64, vp, vp, vp, C.c_int, vp, vp, C.c_int, C.c_int,
                                          C.c_int, C.c_int, vp]

@@ -203,6 +203,8 @@ struct AttnDecodeParams {
   int fuse_rope;
   const bf16* qkv; long long ld_qkv;
   const float* qkv_partial; int qkv_splits; long long qkv_split_stride; long long ld_qkv_partial;
+  const bf16* qkv_bias;   // [ld_qkv] projection bias added to the summed partials before their bf16 rounding (nullptr = none;
+                          // a bf16 `qkv` row already carries it from the GEMM epilogue)
   const bf16* cos_tab; const bf16* sin_tab;
   bf16* kcache_w; bf16* vcache_w;
   // splits > 1: per-(sequence, kv head) arrival counters (zero between launches).  When set, the LAST split CTA to
@@ -291,6 +293,10 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const AttnDec
       if (p.qkv_partial) {
         float a[8];
         sum_partials8(p.qkv_partial + (long long)b * p.ld_qkv_partial + col, p.qkv_splits, p.qkv_split_stride, a);
+        if (p.qkv_bias) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) a[i] += __bfloat162float(p.qkv_bias[col + i]);
+        }
 #pragma unroll
         for (int i = 0; i < 8; ++i) f[i] = bf16_round(a[i]);
       } else {

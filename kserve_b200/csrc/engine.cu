@@ -77,6 +77,7 @@ static int dmalloc(T** p, size_t n) {
 struct LayerW {
   bf16 *wqkv = nullptr, *wo = nullptr, *wgu = nullptr, *wdown = nullptr, *ln1 = nullptr, *ln2 = nullptr;
   bf16 *wr = nullptr, *wgu_e = nullptr, *wdown_e = nullptr;   // MoE: router [E][H], experts [E][2I][H] / [E][H][I]
+  bf16* bqkv = nullptr;   // q/k/v projection bias [qkv_cols] in wqkv's [q | k | v] order (Qwen2); nullptr = none
 };
 
 }  // namespace b200
@@ -351,6 +352,7 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
       GemmArgs a{w.wqkv, e->qkv_cols, e->xn, e->cap_T, e->qkv_cols, B, H, sp > 1 ? EPI_T_PARTIAL : EPI_T_STORE, bn, sp,
                  sp > 1 ? (void*)e->ws : (void*)e->qkv, nullptr, e->qkv_cols, (long long)B * e->qkv_cols, 0, true};
       a.sk_ws = e->sk_ws; a.sk_flags = e->sk_flags; a.sk_tiles = e->sk_tiles; a.sk_ws_floats = e->sk_ws_floats;
+      a.bias = sp > 1 ? nullptr : w.bqkv;   // split-K: the attention prologue adds it to the summed partials
       if ((rc = launch_gemm(e, a, e->num_sms, s))) return rc;
       if (sp > 1) { rp.partial = e->ws; rp.splits = sp; rp.split_stride = (long long)B * e->qkv_cols; rp.ld_partial = e->qkv_cols; }
       rp.qkv = e->qkv;
@@ -369,6 +371,7 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
       GemmArgs a{e->xn + r0 * H, e->cap_T - (int)r0, w.wqkv, e->qkv_cols, T, e->qkv_cols, H, fused_rope ? EPI_ROPE_KV : EPI_STORE, 256, 1,
                  e->qkv + r0 * e->qkv_cols, nullptr, e->qkv_cols, 0, 0, false};
       a.rope = &rp;
+      a.bias = w.bqkv;
       if ((rc = launch_gemm(e, a, gsms, s))) return rc;
     }
     rp.kcache = kc; rp.vcache = vc; rp.page_table = e->d_page_table; rp.max_pages = e->max_pages;
@@ -394,6 +397,7 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
       ap.part_o = e->part_o; ap.part_ml = e->part_ml; ap.scale_log2 = scale_log2;
       ap.fuse_rope = 1; ap.qkv = rp.qkv; ap.ld_qkv = rp.ld; ap.qkv_partial = rp.partial; ap.qkv_splits = rp.splits;
       ap.qkv_split_stride = rp.split_stride; ap.ld_qkv_partial = rp.ld_partial; ap.cos_tab = e->cos_tab; ap.sin_tab = e->sin_tab;
+      ap.qkv_bias = rp.partial ? w.bqkv : nullptr;
       ap.kcache_w = kc; ap.vcache_w = vc;
       static const bool fold = getenv("B200_ATTN_COMBINE_KERNEL") == nullptr;   // =1: separate attn_combine_kernel (A/B)
       ap.split_counter = fold ? e->attn_split_cnt : nullptr;
@@ -1460,7 +1464,7 @@ int b200_engine_destroy(b200_engine_t* e) {
                   e->d_forced, e->d_eos, e->d_stop_tok, e->d_stop_off, e->d_state};
   for (void* p : ptrs) if (p) cudaFree(p);
   for (auto& w : e->layers) {
-    void* lp[] = {w.wqkv, w.wo, w.wgu, w.wdown, w.ln1, w.ln2, w.wr, w.wgu_e, w.wdown_e};
+    void* lp[] = {w.wqkv, w.wo, w.wgu, w.wdown, w.ln1, w.ln2, w.wr, w.wgu_e, w.wdown_e, w.bqkv};
     for (void* p : lp) if (p) cudaFree(p);
   }
   for (auto& kv : e->host_kv) cudaFreeHost(kv.second);
@@ -1528,6 +1532,14 @@ int b200_engine_set_weight(b200_engine_t* e, const char* name, const void* data,
     } else if (rest == "self_attn.v_proj.weight") {
       B200_REQUIRE(expect(KH, H), "shape mismatch for " + n);
       rc = copy_rows(w.wqkv + (ql + kl) * H, src, r * kl, kl, H, dev);
+    } else if (rest == "self_attn.q_proj.bias" || rest == "self_attn.k_proj.bias" || rest == "self_attn.v_proj.bias") {
+      // Qwen2: 1-D biases of the q / k / v projections, sharded by the weights' row ranges, fused in wqkv's order
+      const char which = rest[10];
+      const long long full = which == 'q' ? QH : KH, len = which == 'q' ? ql : kl;
+      const long long off = which == 'q' ? 0 : (which == 'k' ? ql : ql + kl);
+      B200_REQUIRE(expect(full, -1), "shape mismatch for " + n);
+      if (!w.bqkv && (rc = dmalloc(&w.bqkv, (size_t)e->qkv_cols))) return rc;
+      rc = copy_rows(w.bqkv + off, src, r * len, len, 1, dev);
     } else if (rest == "self_attn.o_proj.weight") {
       B200_REQUIRE(expect(H, QH), "shape mismatch for " + n);
       rc = copy_cols(w.wo, src, H, QH, r * ql, ql, dev);
@@ -1573,7 +1585,19 @@ int b200_engine_set_weight(b200_engine_t* e, const char* name, const void* data,
 
 int b200_engine_finalize_weights(b200_engine_t* e) {
   B200_REQUIRE(e, "null engine");
-  const size_t want = 3 + (size_t)e->L * 9;
+  // 3 + 9 L tensors, or 3 + 12 L when every layer also has its q / k / v projection biases (Qwen2); anything in between
+  // is refused: a layer without its bias would run silently wrong
+  size_t nbias = 0;
+  for (const auto& kv : e->seen)
+    if (kv.first.size() > 5 && kv.first.compare(kv.first.size() - 5, 5, ".bias") == 0) ++nbias;
+  if (nbias > 0) {
+    for (int l = 0; l < e->L; ++l)
+      for (const char* pr : {"q", "k", "v"}) {
+        const std::string bn = "model.layers." + std::to_string(l) + ".self_attn." + pr + "_proj.bias";
+        B200_REQUIRE(e->seen.count(bn), "missing weight tensor " + bn + " (q/k/v projection biases must be given for every layer or for none)");
+      }
+  }
+  const size_t want = 3 + (size_t)e->L * (nbias > 0 ? 12 : 9);
   B200_REQUIRE(e->seen.size() == want, "expected " + std::to_string(want) + " weight tensors, got " + std::to_string(e->seen.size()));
   B200_CUDA_OK(cudaDeviceSynchronize());
   e->finalized = true;
@@ -2137,13 +2161,14 @@ static int op_sms() {
   return g_op_sms;
 }
 
-int b200_op_gemm(const void* A, const void* B, void* out, const void* residual, int M, int N, int K, int epi,
-                 int block_n, int splits, int64_t ldo, void* stream) {
+static int op_gemm(const void* A, const void* B, void* out, const void* residual, const void* bias, int M, int N, int K,
+                   int epi, int block_n, int splits, int64_t ldo, void* stream) {
   g_op_tmaps.maps.clear();  // caller buffers may be reused at other shapes
   const bool t = epi >= EPI_T_STORE;
   int out_cols = (epi == EPI_SWIGLU) ? N / 2 : (epi == EPI_T_SWIGLU ? M / 2 : 0);
   GemmArgs a{(const bf16*)A, M, (const bf16*)B, N, M, N, K, epi, block_n, effective_splits(K, splits), out,
              (const bf16*)residual, ldo, (long long)N * ldo, out_cols, t};
+  a.bias = (const bf16*)bias;
   static float* op_sk_ws = nullptr;
   static int* op_sk_flags = nullptr;
   const int op_sk_tiles = 2048;
@@ -2154,6 +2179,17 @@ int b200_op_gemm(const void* A, const void* B, void* out, const void* residual, 
   }
   a.sk_ws = op_sk_ws; a.sk_flags = op_sk_flags; a.sk_tiles = op_sk_tiles; a.sk_ws_floats = (size_t)op_sk_tiles * 2 * 64 * kGemmBlockM;
   return launch_gemm(g_op_tmaps, a, op_sms(), (cudaStream_t)stream);
+}
+
+int b200_op_gemm(const void* A, const void* B, void* out, const void* residual, int M, int N, int K, int epi,
+                 int block_n, int splits, int64_t ldo, void* stream) {
+  return op_gemm(A, B, out, residual, nullptr, M, N, K, epi, block_n, splits, ldo, stream);
+}
+
+int b200_op_gemm_bias(const void* A, const void* B, void* out, const void* residual, int M, int N, int K, int epi,
+                      int block_n, int splits, int64_t ldo, const void* bias, void* stream) {
+  B200_REQUIRE(bias != nullptr && (epi == EPI_STORE || epi == EPI_T_STORE), "b200_op_gemm_bias: a bias with epi 0 or 3");
+  return op_gemm(A, B, out, residual, bias, M, N, K, epi, block_n, splits, ldo, stream);
 }
 
 int b200_op_rmsnorm(void* x, const void* w, void* xn, int rows, int H, float eps, const float* partial, int splits,

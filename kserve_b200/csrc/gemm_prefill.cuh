@@ -51,12 +51,23 @@ __device__ __forceinline__ float2 ld_res2(const bf16* row, int col, int N, bool 
   return r;
 }
 
-// tmap_out: `out` as [rows][out columns] with leading dimension ldo, box [128][64], 128B swizzle; used when p.out_tma
-template <int EPI>
+// bias of output columns (col, col + 1); N bounds the valid columns
+__device__ __forceinline__ float2 ld_bias2(const bf16* b, int col, int N) {
+  float2 r;
+  r.x = col < N ? __bfloat162float(b[col]) : 0.f;
+  r.y = col + 1 < N ? __bfloat162float(b[col + 1]) : 0.f;
+  return r;
+}
+
+// tmap_out: `out` as [rows][out columns] with leading dimension ldo, box [128][64], 128B swizzle; used when p.out_tma.
+// BIAS (EPI_STORE, EPI_ROPE_KV): add p.bias[column] to the fp32 accumulator before its bf16 rounding; a compile-time
+// flag, so the GEMMs without a bias run exactly the code they ran before.
+template <int EPI, bool BIAS = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_prefill_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                     const __grid_constant__ CUtensorMap tmap_out, const GemmParams p) {
   static_assert(EPI == EPI_STORE || EPI == EPI_STORE_RES || EPI == EPI_SWIGLU || EPI == EPI_ROPE_KV, "row-major epilogues only");
+  static_assert(!BIAS || EPI == EPI_STORE || EPI == EPI_ROPE_KV, "bias: QKV epilogues only");
   TraceScope _ts(TK_GEMM + 100 * EPI + 1000 * (p.M >> 7));
   using Cfg = PrefillCfg<EPI>;
   constexpr int STAGES = Cfg::kStages;
@@ -173,9 +184,11 @@ gemm_prefill_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
 #pragma unroll
       for (int j = 0; j < BLOCK_N / 8; ++j) {
         const int col = 8 * j + 2 * qd;
+        const float2 bb = BIAS ? ld_bias2(p.bias + n0, col, p.N - n0) : make_float2(0.f, 0.f);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           float f0 = accum[4 * j + 2 * h], f1 = accum[4 * j + 2 * h + 1];
+          if constexpr (BIAS) { f0 += bb.x; f1 += bb.y; }
           if constexpr (EPI == EPI_STORE_RES) {
             if (rrow[h] != nullptr) {
               const float2 r2 = ld_res2(rrow[h], col, p.N - n0, rpair);
@@ -206,7 +219,8 @@ gemm_prefill_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
           }
         }
     } else {   // EPI_ROPE_KV: the tile is heads 2 n_t, 2 n_t + 1 of [q heads | k heads | v heads] x 128
-      // HF bf16 rounding points of apply_rotary_pos_emb (bit-identical to rope_kv_kernel)
+      // HF bf16 rounding points of apply_rotary_pos_emb (bit-identical to rope_kv_kernel); the projection bias is added
+      // to the fp32 accumulator before its one bf16 rounding, i.e. before the rotation as in HF
       int pos[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -216,23 +230,34 @@ gemm_prefill_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         const int head = 2 * n_t + hh;
+        const bool hb = BIAS && head < p.rope_nh + 2 * p.rope_nkv;   // (uniform; past the last head there is no bias)
         if (head >= p.rope_nh + p.rope_nkv) {   // v head (or past the last head): copied as is
 #pragma unroll
-          for (int j = 16 * hh; j < 16 * hh + 16; ++j)
+          for (int j = 16 * hh; j < 16 * hh + 16; ++j) {
+            const float2 bb = hb ? ld_bias2(p.bias + n0, 8 * j + 2 * qd, p.N - n0) : make_float2(0.f, 0.f);
 #pragma unroll
-            for (int h = 0; h < 2; ++h)
-              st_shared_u32(ot + out_tile_off(frag_row + 8 * h, 8 * j + 2 * qd), pack_bf16x2(accum[4 * j + 2 * h], accum[4 * j + 2 * h + 1]));
+            for (int h = 0; h < 2; ++h) {
+              float f0 = accum[4 * j + 2 * h], f1 = accum[4 * j + 2 * h + 1];
+              if (hb) { f0 += bb.x; f1 += bb.y; }
+              st_shared_u32(ot + out_tile_off(frag_row + 8 * h, 8 * j + 2 * qd), pack_bf16x2(f0, f1));
+            }
+          }
         } else {                                  // q or k head: rotate-half RoPE on the pairs (d, d + 64)
 #pragma unroll
           for (int jj = 0; jj < 8; ++jj) {
             const int j1 = 16 * hh + jj, j2 = j1 + 8;
             const int d = 8 * jj + 2 * qd;
+            const float2 ba = hb ? ld_bias2(p.bias + n0, 8 * j1 + 2 * qd, p.N - n0) : make_float2(0.f, 0.f);
+            const float2 bc = hb ? ld_bias2(p.bias + n0, 8 * j2 + 2 * qd, p.N - n0) : make_float2(0.f, 0.f);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               const float2 cs = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.rope_cos + (long long)pos[h] * 64 + d));
               const float2 sn = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.rope_sin + (long long)pos[h] * 64 + d));
-              const float a0 = bf16_round(accum[4 * j1 + 2 * h]), a1 = bf16_round(accum[4 * j1 + 2 * h + 1]);
-              const float b0 = bf16_round(accum[4 * j2 + 2 * h]), b1 = bf16_round(accum[4 * j2 + 2 * h + 1]);
+              float x0 = accum[4 * j1 + 2 * h], x1 = accum[4 * j1 + 2 * h + 1];
+              float y0 = accum[4 * j2 + 2 * h], y1 = accum[4 * j2 + 2 * h + 1];
+              if (hb) { x0 += ba.x; x1 += ba.y; y0 += bc.x; y1 += bc.y; }
+              const float a0 = bf16_round(x0), a1 = bf16_round(x1);
+              const float b0 = bf16_round(y0), b1 = bf16_round(y1);
               const float o1x = bf16_round(a0 * cs.x) + bf16_round(-b0 * sn.x);
               const float o1y = bf16_round(a1 * cs.y) + bf16_round(-b1 * sn.y);
               const float o2x = bf16_round(b0 * cs.x) + bf16_round(a0 * sn.x);

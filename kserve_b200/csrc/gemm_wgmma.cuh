@@ -16,10 +16,10 @@
 namespace b200 {
 
 enum GemmEpi : int {
-  EPI_STORE = 0,      // out[m][n] = bf16(acc)
+  EPI_STORE = 0,      // out[m][n] = bf16(acc [+ bias[n]])
   EPI_STORE_RES = 1,  // out[m][n] = bf16(bf16(acc) + residual[m][n])           (o_proj / down_proj + residual)
   EPI_SWIGLU = 2,     // B rows interleaved {16 gate,16 up}: out[m][n/2] = bf16(bf16(silu(g)) * u)
-  EPI_T_STORE = 3,    // out[n][m] = bf16(acc)                                    (swap-AB)
+  EPI_T_STORE = 3,    // out[n][m] = bf16(acc [+ bias[m]])                        (swap-AB)
   EPI_T_SWIGLU = 4,   // A rows interleaved {16 gate,16 up}: out[n][m/2] = ...    (swap-AB)
   EPI_T_PARTIAL = 5,  // ws[split][n][m] = acc (fp32)                             (swap-AB split-K)
   EPI_ROPE_KV = 6,    // prefill QKV projection (BLOCK_N 256): columns are [q heads | k heads | v heads] x 128;
@@ -69,6 +69,9 @@ struct GemmParams {
   int sk_slots;            // partial slots per tile
   float* sk_ws;            // [m_tiles][sk_slots][BLOCK_N][128] fp32
   int* sk_flags;           // [m_tiles] arrival counters, 0 between launches
+  // per-output-feature bias (EPI_STORE, EPI_ROPE_KV: column n; EPI_T_STORE: weight row m), nullptr = none.  It is added
+  // in fp32 to the finished accumulator, so the output is ONE bf16 rounding of (acc + bias) as nn.Linear(bias=True) gives.
+  const bf16* bias;
 };
 
 constexpr int kGemmBlockM = 128;
@@ -374,6 +377,11 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           }
           if constexpr (EPI == EPI_T_STORE) {
             if (m < M_rt) {
+              if (p.bias != nullptr) {   // after the stream-K pieces are in: one code point for plain and stream-K tiles
+                const float bm = __bfloat162float(p.bias[m]);
+#pragma unroll
+                for (int j = 0; j < CH; ++j) v[j] += bm;
+              }
               bf16* o = reinterpret_cast<bf16*>(p.out) + out_off + (long long)(n0 + c0 + roff_b) * p.ldo + m;
 #pragma unroll
               for (int j = 0; j < CH; ++j)

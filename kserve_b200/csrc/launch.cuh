@@ -108,10 +108,10 @@ inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_
   return cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
 }
 
-template <int EPI>
+template <int EPI, bool BIAS = false>
 int launch_prefill_inst(const CUtensorMap* ta, const CUtensorMap* tb, const CUtensorMap* to, const GemmParams& p, int grid,
                         cudaStream_t s) {
-  auto kern = gemm_prefill_kernel<EPI>;
+  auto kern = gemm_prefill_kernel<EPI, BIAS>;
   static bool configured = false;  // per instantiation
   if (!configured) {
     B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PrefillCfg<EPI>::kSmemBytes));
@@ -161,6 +161,7 @@ struct GemmArgs {
   long long group_out_stride = 0;   // n_rt / row_off are arrays of `groups` entries
   PfCtx* pf = nullptr;              // weight-stream prefetcher context of the step being enqueued (decode only)
   const RopeKvParams* rope = nullptr;   // EPI_ROPE_KV: where RoPE(k) / v go and the tables (q is rotated in place in `out`)
+  const bf16* bias = nullptr;       // per-output-feature bias (EPI_STORE, EPI_ROPE_KV, EPI_T_STORE), see GemmParams::bias
 };
 
 // GEMMs whose weight operand depends on nothing the step computes (decode swap-AB, no device-side extents)
@@ -227,6 +228,9 @@ inline int launch_gemm(TmapCache& cache, const GemmArgs& a, int num_sms, cudaStr
     a.pf->count++;
   }
   B200_REQUIRE(p.splits == 1 || a.epi == EPI_T_PARTIAL, "split-K only with the fp32 partial epilogue");
+  B200_REQUIRE(!a.bias || ((a.epi == EPI_STORE || a.epi == EPI_ROPE_KV || a.epi == EPI_T_STORE) && a.groups == 0),
+               "a GEMM bias needs the EPI_STORE, EPI_ROPE_KV or EPI_T_STORE epilogue of an ungrouped GEMM");
+  p.bias = a.bias;
   p.rope_tok_seq = nullptr; p.rope_tok_pos = nullptr; p.rope_page_table = nullptr; p.rope_max_pages = 0;
   p.rope_kcache = nullptr; p.rope_vcache = nullptr; p.rope_cos = nullptr; p.rope_sin = nullptr; p.rope_nh = 0; p.rope_nkv = 0;
   if (a.epi == EPI_ROPE_KV) {
@@ -249,10 +253,12 @@ inline int launch_gemm(TmapCache& cache, const GemmArgs& a, int num_sms, cudaStr
       if ((rc = cache.get(a.out, out_rows, out_cols, kGemmBlockM, &to, (uint64_t)a.ldo))) return rc;
       p.out_tma = 1;
     }
-    if (a.epi == EPI_STORE) return launch_prefill_inst<EPI_STORE>(ta, tb, to, p, grid, s);
+    if (a.epi == EPI_STORE) return a.bias ? launch_prefill_inst<EPI_STORE, true>(ta, tb, to, p, grid, s)
+                                          : launch_prefill_inst<EPI_STORE>(ta, tb, to, p, grid, s);
     if (a.epi == EPI_STORE_RES) return launch_prefill_inst<EPI_STORE_RES>(ta, tb, to, p, grid, s);
     if (a.epi == EPI_SWIGLU) return launch_prefill_inst<EPI_SWIGLU>(ta, tb, to, p, grid, s);
-    return launch_prefill_inst<EPI_ROPE_KV>(ta, tb, to, p, grid, s);
+    return a.bias ? launch_prefill_inst<EPI_ROPE_KV, true>(ta, tb, to, p, grid, s)
+                  : launch_prefill_inst<EPI_ROPE_KV>(ta, tb, to, p, grid, s);
   }
 #define B200_GEMM_CASE(BN, E) \
   if (a.block_n == BN && a.epi == E) return launch_gemm_inst<BN, E>(ta, tb, p, grid, s);

@@ -151,8 +151,14 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
                 self.model_config = json.load(f)
         cfg = self.model_config
         arch = (cfg.get("architectures") or ["LlamaForCausalLM"])[0]
-        if not arch.endswith("ForCausalLM") or cfg.get("model_type", "llama") not in ("llama", "mistral", "mixtral"):
-            raise OpenAIError(f"architecture {arch} is not supported by the H100 runtime (Llama / Mistral / Mixtral decoders only)")
+        model_type = cfg.get("model_type", "llama")
+        if not arch.endswith("ForCausalLM") or model_type not in ("llama", "mistral", "mixtral", "qwen2"):
+            raise OpenAIError(f"architecture {arch} is not supported by the H100 runtime "
+                              "(Llama / Mistral / Mixtral / Qwen2 decoders only)")
+        head_dim = cfg.get("head_dim") or cfg["hidden_size"] // cfg["num_attention_heads"]
+        if head_dim != 128:
+            # (Qwen2-0.5B, Qwen2.5-0.5B, Llama-3.2-1B: the KV page layout and both attention kernels are built for 128)
+            raise OpenAIError(f"head_dim={head_dim} is not supported by the H100 runtime (head_dim 128 only)")
         if self._tokenizer is None and self.model_id_or_path and os.path.exists(
                 os.path.join(self.model_id_or_path, "tokenizer.json")):
             from transformers import AutoTokenizer
@@ -182,6 +188,8 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
             logger.warning("sliding_window=%d < max length %d: serving at most %d tokens (full attention == sliding "
                            "window inside the window)", window, self.max_length, window)
             self.max_length = int(window)
+        # Qwen2's q / k / v biases are implied by its architecture (they come with the checkpoint); a Llama
+        # attention_bias would also put one on o_proj, which the engine does not have
         for key in ("attention_bias", "mlp_bias"):
             if cfg.get(key):
                 raise OpenAIError(f"config.{key}=true is not supported by the H100 runtime")

@@ -1,16 +1,18 @@
 """Llama-family tensor table: HF state_dict names and shapes the engine expects
-(what AutoModelForCausalLM.from_pretrained loads in the reference, generative_model.py:249-254)."""
+(what AutoModelForCausalLM.from_pretrained loads in the reference, generative_model.py:249-254).
+Qwen2 configs (model_type "qwen2") add the q / k / v projection biases, and a tied checkpoint has no lm_head.weight."""
 from __future__ import annotations
 
 from typing import Iterator, Tuple
 
 
 def llama_tensor_specs(cfg: dict) -> Iterator[Tuple[str, Tuple[int, ...], str]]:
-    """Yield (name, shape, kind); kind in {embed, linear, norm}."""
+    """Yield (name, shape, kind); kind in {embed, linear, norm, bias}."""
     H, I, V = cfg["hidden_size"], cfg["intermediate_size"], cfg["vocab_size"]
     nh, nkv = cfg["num_attention_heads"], cfg["num_key_value_heads"]
     d = cfg.get("head_dim") or H // nh
     E = int(cfg.get("num_local_experts", 0) or 0)
+    qwen2 = cfg.get("model_type") == "qwen2"
     yield "model.embed_tokens.weight", (V, H), "embed"
     for i in range(cfg["num_hidden_layers"]):
         if E:   # Mixtral-style sparse MoE (transformers 5.x fused-expert state_dict)
@@ -28,12 +30,19 @@ def llama_tensor_specs(cfg: dict) -> Iterator[Tuple[str, Tuple[int, ...], str]]:
         p = f"model.layers.{i}."
         yield p + "input_layernorm.weight", (H,), "norm"
         yield p + "self_attn.q_proj.weight", (nh * d, H), "linear"
+        if qwen2:
+            yield p + "self_attn.q_proj.bias", (nh * d,), "bias"
         yield p + "self_attn.k_proj.weight", (nkv * d, H), "linear"
+        if qwen2:
+            yield p + "self_attn.k_proj.bias", (nkv * d,), "bias"
         yield p + "self_attn.v_proj.weight", (nkv * d, H), "linear"
+        if qwen2:
+            yield p + "self_attn.v_proj.bias", (nkv * d,), "bias"
         yield p + "self_attn.o_proj.weight", (H, nh * d), "linear"
         yield p + "post_attention_layernorm.weight", (H,), "norm"
         yield p + "mlp.gate_proj.weight", (I, H), "linear"
         yield p + "mlp.up_proj.weight", (I, H), "linear"
         yield p + "mlp.down_proj.weight", (H, I), "linear"
     yield "model.norm.weight", (H,), "norm"
-    yield "lm_head.weight", (V, H), "linear"
+    if not cfg.get("tie_word_embeddings"):
+        yield "lm_head.weight", (V, H), "linear"

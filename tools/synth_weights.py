@@ -71,6 +71,31 @@ CONFIGS["tiny_g2_rope3"] = dict(CONFIGS["tiny_g2"], max_position_embeddings=4096
 for _base in ("tiny_g2", "tiny_g4", "tiny_kv8", "llama3_8b_2l"):
     CONFIGS[_base + "_peaked"] = dict(CONFIGS[_base], _peaked=True)
 
+# Qwen2 / Qwen2.5 decoders: Llama layers plus q / k / v projection biases (theta 1e6, eps 1e-6).  GQA groups 7, 6 and 5
+# are those of Qwen2-0.5B / Qwen2.5-3B / Qwen2.5-32B.  tiny_qwen2's decode QKV projection (18 m-tiles) takes split-K;
+# tiny_qwen2_wide's (qkv_cols 10240 = 80 m-tiles) takes the bf16 EPI_T_STORE epilogue, as 72B-class models do.
+_QWEN2 = dict(model_type="qwen2", head_dim=128, max_position_embeddings=2048, rms_norm_eps=1e-6, rope_theta=1000000.0,
+              use_sliding_window=False)
+QWEN2_CONFIGS: Dict[str, dict] = {
+    "tiny_qwen2": dict(_QWEN2, vocab_size=1031, hidden_size=896, intermediate_size=4864, num_hidden_layers=2,
+                       num_attention_heads=14, num_key_value_heads=2),
+    "tiny_qwen2_g6_tied": dict(_QWEN2, vocab_size=1031, hidden_size=768, intermediate_size=2048, num_hidden_layers=2,
+                               num_attention_heads=12, num_key_value_heads=2, tie_word_embeddings=True),
+    "tiny_qwen2_g5": dict(_QWEN2, vocab_size=1031, hidden_size=640, intermediate_size=1536, num_hidden_layers=2,
+                          num_attention_heads=10, num_key_value_heads=2),
+    "tiny_qwen2_wide": dict(_QWEN2, vocab_size=1031, hidden_size=512, intermediate_size=1024, num_hidden_layers=2,
+                            num_attention_heads=64, num_key_value_heads=8),
+    # Qwen2.5-7B layer and vocabulary shapes, 2 layers
+    "qwen2_7b_2l": dict(_QWEN2, vocab_size=152064, hidden_size=3584, intermediate_size=18944, num_hidden_layers=2,
+                        num_attention_heads=28, num_key_value_heads=4, max_position_embeddings=32768),
+    # Qwen2.5-7B, all 28 layers (tools/model_bench.py)
+    "qwen2_7b": dict(_QWEN2, vocab_size=152064, hidden_size=3584, intermediate_size=18944, num_hidden_layers=28,
+                     num_attention_heads=28, num_key_value_heads=4, max_position_embeddings=32768),
+}
+for _base in ("tiny_qwen2", "qwen2_7b_2l"):
+    QWEN2_CONFIGS[_base + "_peaked"] = dict(QWEN2_CONFIGS[_base], _peaked=True)
+CONFIGS.update(QWEN2_CONFIGS)
+
 
 def hf_config_dict(cfg: dict) -> dict:
     """the keys a transformers config understands (drops this module's private `_...` markers)"""
@@ -98,26 +123,45 @@ def moe_tensor_specs(cfg: dict) -> Iterator[Tuple[str, Tuple[int, ...], str]]:
 
 
 def tensor_specs(cfg: dict) -> Iterator[Tuple[str, Tuple[int, ...], str]]:
-    """Yield (name, shape, kind) in canonical order. kind in {embed, linear, norm}."""
+    """Yield (name, shape, kind) in canonical order. kind in {embed, linear, norm, bias}.  Qwen2 biases follow their
+    weight, and a tied checkpoint has no lm_head.weight; the Llama / Mixtral order (and so every seed) is unchanged."""
     H, I, V = cfg["hidden_size"], cfg["intermediate_size"], cfg["vocab_size"]
     nh, nkv, d = cfg["num_attention_heads"], cfg["num_key_value_heads"], cfg["head_dim"]
     if "num_local_experts" in cfg:
         yield from moe_tensor_specs(cfg)
         return
+    qwen2 = cfg.get("model_type") == "qwen2"
     yield "model.embed_tokens.weight", (V, H), "embed"
     for i in range(cfg["num_hidden_layers"]):
         p = f"model.layers.{i}."
         yield p + "input_layernorm.weight", (H,), "norm"
-        yield p + "self_attn.q_proj.weight", (nh * d, H), "linear"
-        yield p + "self_attn.k_proj.weight", (nkv * d, H), "linear"
-        yield p + "self_attn.v_proj.weight", (nkv * d, H), "linear"
+        for proj, rows in (("q", nh * d), ("k", nkv * d), ("v", nkv * d)):
+            yield p + f"self_attn.{proj}_proj.weight", (rows, H), "linear"
+            if qwen2:
+                yield p + f"self_attn.{proj}_proj.bias", (rows,), "bias"
         yield p + "self_attn.o_proj.weight", (H, nh * d), "linear"
         yield p + "post_attention_layernorm.weight", (H,), "norm"
         yield p + "mlp.gate_proj.weight", (I, H), "linear"
         yield p + "mlp.up_proj.weight", (I, H), "linear"
         yield p + "mlp.down_proj.weight", (H, I), "linear"
     yield "model.norm.weight", (H,), "norm"
-    yield "lm_head.weight", (V, H), "linear"
+    if not cfg.get("tie_word_embeddings"):
+        yield "lm_head.weight", (V, H), "linear"
+
+
+def synth_bias(index: int, shape, name: str, seed: int, dtype=torch.bfloat16) -> torch.Tensor:
+    """Qwen2 q / k / v biases.  HF initialises them to zero, so they are drawn large enough that a dropped, doubled or
+    misplaced (after RoPE) bias moves the logits: q, v ~ N(0, 0.5); k ~ N(0, 2) with a few entries near +-20, the
+    outliers real Qwen k biases have."""
+    g = torch.Generator(device="cpu")
+    g.manual_seed(seed * 1000003 + index * 7919 + 17)
+    if ".k_proj." in name:
+        t = 2.0 * torch.randn(shape, generator=g, dtype=torch.float32)
+        idx = torch.randperm(shape[0], generator=g)[: max(2, shape[0] // 64)]
+        t[idx] = torch.sign(t[idx] + 1e-3) * (18.0 + 4.0 * torch.rand(idx.shape, generator=g))
+    else:
+        t = 0.5 * torch.randn(shape, generator=g, dtype=torch.float32)
+    return t.to(dtype)
 
 
 def synth_tensor(index: int, shape, kind: str, seed: int, dtype=torch.bfloat16) -> torch.Tensor:
@@ -147,6 +191,9 @@ def iter_state_dict(cfg: dict, seed: int = 0, dtype=torch.bfloat16):
             embed = synth_tensor(0, shape, "embed", seed, dtype)      # index 0 == model.embed_tokens.weight
             yield name, embed[peaked_perm(shape[0], seed)].contiguous()
             continue
+        if kind == "bias":
+            yield name, synth_bias(idx, shape, name, seed, dtype)
+            continue
         yield name, synth_tensor(idx, shape, kind, seed, dtype)
 
 
@@ -161,6 +208,6 @@ def checksum(sd: Dict[str, torch.Tensor]) -> float:
     if third not in sd:   # MoE checkpoints have fused expert tensors instead
         third = "model.layers.0.self_attn.o_proj.weight"
     for name in ("model.embed_tokens.weight", "lm_head.weight", third):
-        t = sd[name]
+        t = sd[name] if name in sd else sd["model.embed_tokens.weight"]   # (tied checkpoints have no lm_head.weight)
         s += float(t[: 64].float().sum()) + float(t[-1].float().abs().sum())
     return s
