@@ -45,6 +45,9 @@ typedef struct b200_model_config {
   int32_t device;              /* CUDA device ordinal */
   int32_t num_experts;         /* 0 = dense MLP; > 0 = Mixtral-style sparse MoE (modeling_mixtral.py:62-135) */
   int32_t num_experts_per_tok; /* must be 2 when num_experts > 0 */
+  int32_t weight_format;       /* 0 = bf16; 1 = FP8: the q/k/v/o and gate/up/down projections are float8_e4m3fn codes with
+                                * one scale per weight row (b200_engine_set_weight_fp8); dense models on one GPU only
+                                * (tp_size 1) */
 } b200_model_config_t;
 
 /* Creates the engine on cfg->device. nccl_unique_id: 128 bytes shared by all ranks (from
@@ -71,6 +74,16 @@ int b200_engine_ipc_import(b200_engine_t* e, const void* handles, int32_t n);
  * all three biases. */
 int b200_engine_set_weight(b200_engine_t* e, const char* hf_name, const void* data, int on_device,
                            int ndim, const int64_t* shape);
+/* weight_format 1: the seven projection weights `model.layers.N.{self_attn.{q,k,v,o}_proj, mlp.{gate,up,down}_proj}.weight`
+ * as FULL (unsharded) float8_e4m3fn codes [out][in] plus `scale`, one value per output row ([out]; a per-tensor scale is
+ * broadcast by the caller), bf16 (scale_dtype 0) or fp32 (1, rounded to bf16 here).  The two NaN codes (0x7F, 0xFF) must
+ * not occur (the Python loader refuses them): the engine expands them to +-480 * scale, not NaN.  Both on the host or both on this
+ * engine's GPU (on_device).  The engine multiplies exactly W' = bf16(code) * bf16(scale), rounded once to bf16 — the
+ * operand compressed-tensors' decompression gives transformers — so it is bit-identical to a bf16 engine loaded with W'.
+ * Decode streams the codes (one byte per weight); prefill dequantizes one layer at a time into a bf16 scratch.
+ * b200_engine_set_weight refuses these seven names on an FP8 engine; every other tensor stays bf16. */
+int b200_engine_set_weight_fp8(b200_engine_t* e, const char* hf_name, const void* data, const void* scale,
+                               int scale_dtype, int on_device, int ndim, const int64_t* shape);
 int b200_engine_finalize_weights(b200_engine_t* e);
 /* Optional: bf16 cos/sin tables [max_position][64] computed by the host exactly as
  * LlamaRotaryEmbedding.forward does (fp32 inv_freq * position -> cos/sin -> bf16).  Without this call the
@@ -177,6 +190,12 @@ int b200_op_gemm(const void* A, const void* B, void* out, const void* residual, 
  * epi 0 (block_n 256) adds bias[n] to out[m][n], epi 3 (block_n 16/32/64) adds bias[m] to out[n][m]. */
 int b200_op_gemm_bias(const void* A, const void* B, void* out, const void* residual, int M, int N, int K, int epi,
                       int block_n, int splits, int64_t ldo, const void* bias, void* stream);
+/* b200_op_gemm's swap-AB kernel (epi 3-5, block_n 16/32/64) with FP8 weights: A8 = float8_e4m3fn [M,K] (K % 16 == 0),
+ * scale = bf16 [M]; bias (epi 3 only) may be NULL.  Equals b200_op_gemm on W' = b200_op_dequant_fp8(A8, scale) bit for bit. */
+int b200_op_gemm_fp8(const void* A8, const void* scale, const void* B, void* out, const void* bias, int M, int N, int K,
+                     int epi, int block_n, int splits, int64_t ldo, void* stream);
+/* out[r][k] = bf16(code[r][k]) * scale[r] rounded once to bf16 (bf16 [rows,K]); K % 16 == 0, 16-byte aligned buffers */
+int b200_op_dequant_fp8(const void* q, const void* scale, void* out, int64_t rows, int K, void* stream);
 int b200_op_rmsnorm(void* x, const void* w, void* xn, int rows, int H, float eps, const float* partial,
                     int splits, const void* y, void* stream);
 int b200_op_attn_prefill(const void* q, int64_t ldq, void* out, int64_t ldo, const void* kcache,

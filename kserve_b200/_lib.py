@@ -14,7 +14,7 @@ class ModelConfig(C.Structure):
         "vocab_size", "hidden_size", "intermediate_size", "num_layers", "num_heads", "num_kv_heads",
         "head_dim", "max_position")] + [("rms_eps", C.c_float), ("rope_theta", C.c_float)] + [
         (n, C.c_int32) for n in ("max_batch", "max_seq_len", "max_prefill_tokens", "num_kv_pages",
-                                 "tp_rank", "tp_size", "device", "num_experts", "num_experts_per_tok")]
+                                 "tp_rank", "tp_size", "device", "num_experts", "num_experts_per_tok", "weight_format")]
 
 
 class GenParams(C.Structure):
@@ -55,6 +55,7 @@ def load() -> C.CDLL:
     lib.b200_engine_destroy.argtypes = [vp]
     lib.b200_nccl_unique_id.argtypes = [vp]
     lib.b200_engine_set_weight.argtypes = [vp, C.c_char_p, vp, C.c_int, C.c_int, C.POINTER(i64)]
+    lib.b200_engine_set_weight_fp8.argtypes = [vp, C.c_char_p, vp, vp, C.c_int, C.c_int, C.c_int, C.POINTER(i64)]
     lib.b200_engine_finalize_weights.argtypes = [vp]
     lib.b200_engine_set_rope_table.argtypes = [vp, vp, vp, i32]
     lib.b200_generate.argtypes = [vp, vp, vp, i32, i32, C.POINTER(GenParams), vp, C.POINTER(i32),
@@ -67,6 +68,8 @@ def load() -> C.CDLL:
     lib.b200_fetch_staged.argtypes = [vp, vp, C.POINTER(i32), C.POINTER(i32)]
     lib.b200_op_gemm.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, i64, vp]
     lib.b200_op_gemm_bias.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, i64, vp, vp]
+    lib.b200_op_gemm_fp8.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, i64, vp]
+    lib.b200_op_dequant_fp8.argtypes = [vp, vp, vp, i64, C.c_int, vp]
     lib.b200_op_rmsnorm.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_float, vp, C.c_int, vp, vp]
     lib.b200_op_attn_prefill.argtypes = [vp, i64, vp, i64, vp, vp, vp, C.c_int, vp, vp, C.c_int, C.c_int,
                                          C.c_int, C.c_int, vp]

@@ -78,6 +78,10 @@ struct LayerW {
   bf16 *wqkv = nullptr, *wo = nullptr, *wgu = nullptr, *wdown = nullptr, *ln1 = nullptr, *ln2 = nullptr;
   bf16 *wr = nullptr, *wgu_e = nullptr, *wdown_e = nullptr;   // MoE: router [E][H], experts [E][2I][H] / [E][H][I]
   bf16* bqkv = nullptr;   // q/k/v projection bias [qkv_cols] in wqkv's [q | k | v] order (Qwen2); nullptr = none
+  // weight_format 1: the four projections as e4m3 codes in the bf16 matrices' layouts (the bf16 pointers above stay null)
+  // and the bf16 scale of every fused row (o / down: all H rows on every rank)
+  uint8_t *wqkv8 = nullptr, *wo8 = nullptr, *wgu8 = nullptr, *wdown8 = nullptr;
+  bf16 *sqkv = nullptr, *so = nullptr, *sgu = nullptr, *sdown = nullptr;
 };
 
 }  // namespace b200
@@ -102,6 +106,8 @@ struct b200_engine {
   // weights
   bf16 *embed = nullptr, *lm_head = nullptr, *final_norm = nullptr;
   std::vector<LayerW> layers;
+  bool fp8 = false;                          // cfg.weight_format == 1
+  bf16* wdq = nullptr;                       // FP8 prefill: the current layer's projections dequantized to bf16
   std::unordered_map<std::string, int> seen;
   bool finalized = false;
   bf16 *cos_tab = nullptr, *sin_tab = nullptr;
@@ -338,7 +344,28 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
     const int T = vw.T, B = vw.B;
     const long long r0 = vw.r0;        // first row of this micro-batch in the packed activation buffers (0 in decode)
     cudaStream_t s = vw.s;
-    const LayerW& w = e->layers[l];
+    LayerW w = e->layers[l];   // (a copy: FP8 prefill points the bf16 matrices at the layer's dequantized scratch)
+    if (e->fp8 && !decode) {
+      // the prefill GEMMs are compute-bound: they run unchanged on W' = dequant(codes, scales), expanded once per layer
+      // into one scratch (one stream: FP8 engines are single-GPU, so there is no second micro-batch stream)
+      bf16* base = e->wdq;
+      const long long H_ = H, QH = (long long)e->nh * kHeadDim, I_ = e->I;
+      {
+        Fp8Segs sg{};
+        const LayerW& q = e->layers[l];
+        sg.seg[0] = Fp8Seg{q.wqkv8, q.sqkv, base, (long long)e->qkv_cols * H_ / 16, H};
+        sg.seg[1] = Fp8Seg{q.wo8, q.so, base + (long long)e->qkv_cols * H_, H_ * QH / 16, (int)QH};
+        sg.seg[2] = Fp8Seg{q.wgu8, q.sgu, base + (long long)e->qkv_cols * H_ + H_ * QH, 2 * I_ * H_ / 16, H};
+        sg.seg[3] = Fp8Seg{q.wdown8, q.sdown, base + (long long)e->qkv_cols * H_ + H_ * QH + 2 * I_ * H_, H_ * I_ / 16, e->I};
+        sg.n = 4;
+        if ((rc = launch_dequant_fp8(sg, s))) return rc;
+        e->launches++;
+      }
+      w.wqkv = base;
+      w.wo = base + (long long)e->qkv_cols * H_;
+      w.wgu = w.wo + H_ * QH;
+      w.wdown = w.wgu + 2 * I_ * H_;
+    }
     bf16* kc = e->kcache + (long long)l * e->layer_stride;
     bf16* vc = e->vcache + (long long)l * e->layer_stride;
     // ---- QKV projection
@@ -353,6 +380,7 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
                  sp > 1 ? (void*)e->ws : (void*)e->qkv, nullptr, e->qkv_cols, (long long)B * e->qkv_cols, 0, true};
       a.sk_ws = e->sk_ws; a.sk_flags = e->sk_flags; a.sk_tiles = e->sk_tiles; a.sk_ws_floats = e->sk_ws_floats;
       a.bias = sp > 1 ? nullptr : w.bqkv;   // split-K: the attention prologue adds it to the summed partials
+      a.a8 = w.wqkv8; a.a_scale = w.sqkv;
       if ((rc = launch_gemm(e, a, e->num_sms, s))) return rc;
       if (sp > 1) { rp.partial = e->ws; rp.splits = sp; rp.split_stride = (long long)B * e->qkv_cols; rp.ld_partial = e->qkv_cols; }
       rp.qkv = e->qkv;
@@ -422,12 +450,14 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
       e->launches++;
     }
     // ---- row-parallel projections (o_proj, down_proj) followed by residual add + next RMSNorm
-    auto row_parallel = [&](const bf16* act, int K, const bf16* wmat, const bf16* next_norm) -> int {
+    auto row_parallel = [&](const bf16* act, int K, const bf16* wmat, const uint8_t* wmat8, const bf16* wscale,
+                            const bf16* next_norm) -> int {
       int rc2;
       if (decode) {
         const int sp = pick_splits(e, H, K);
         if (sp > 1) {
           GemmArgs a{wmat, H, act, e->cap_T, H, B, K, EPI_T_PARTIAL, bn, sp, e->ws, nullptr, H, (long long)B * H, 0, true};
+          a.a8 = wmat8; a.a_scale = wscale;
           if ((rc2 = launch_gemm(e, a, e->num_sms, s))) return rc2;
           e->launches++;
           if (!tp) {
@@ -447,6 +477,7 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
         } else {
           GemmArgs a{wmat, H, act, e->cap_T, H, B, K, EPI_T_STORE, bn, 1, e->ybuf, nullptr, H, 0, 0, true};
           a.sk_ws = e->sk_ws; a.sk_flags = e->sk_flags; a.sk_tiles = e->sk_tiles; a.sk_ws_floats = e->sk_ws_floats;
+          a.a8 = wmat8; a.a_scale = wscale;
           if ((rc2 = launch_gemm(e, a, e->num_sms, s))) return rc2;
           e->launches++;
           if (tp && e->p2p_ready) {
@@ -474,7 +505,7 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
       e->launches++;
       return 0;
     };
-    if ((rc = row_parallel(e->attn, e->nh * kHeadDim, w.wo, w.ln2))) return rc;
+    if ((rc = row_parallel(e->attn, e->nh * kHeadDim, w.wo, w.wo8, w.so, w.ln2))) return rc;
     const bf16* next_norm = (l + 1 < e->L) ? e->layers[l + 1].ln1 : e->final_norm;
     if (e->E > 0) {
       // ---- sparse MoE: route, group rows per expert, run the expert GEMMs bounded by the device-side counts, combine
@@ -555,6 +586,7 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
       if (gsp > 1) {   // few tiles per GPU (tensor parallel): split-K partials + a reducing SwiGLU kernel
         GemmArgs a{w.wgu, 2 * e->I, e->xn, e->cap_T, 2 * e->I, B, H, EPI_T_PARTIAL, bn, gsp, e->ws, nullptr, 2 * e->I,
                    (long long)B * 2 * e->I, 0, true};
+        a.a8 = w.wgu8; a.a_scale = w.sgu;
         if ((rc = launch_gemm(e, a, e->num_sms, s))) return rc;
         B200_CUDA_OK(launch_k(swiglu_reduce_kernel, dim3(B), dim3(512), 0, s, (const float*)e->ws, gsp, (long long)B * 2 * e->I,
                               (long long)2 * e->I, e->hbuf, e->I));
@@ -562,6 +594,7 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
       } else {
         GemmArgs a{w.wgu, 2 * e->I, e->xn, e->cap_T, 2 * e->I, B, H, EPI_T_SWIGLU, bn, 1, e->hbuf, nullptr, e->I, 0, e->I, true};
         a.sk_ws = e->sk_ws; a.sk_flags = e->sk_flags; a.sk_tiles = e->sk_tiles; a.sk_ws_floats = e->sk_ws_floats;
+        a.a8 = w.wgu8; a.a_scale = w.sgu;
         if ((rc = launch_gemm(e, a, e->num_sms, s))) return rc;
       }
     } else {
@@ -569,7 +602,7 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
       if ((rc = launch_gemm(e, a, gsms, s))) return rc;
     }
     e->launches++;
-    if ((rc = row_parallel(e->hbuf, e->I, w.wdown, next_norm))) return rc;
+    if ((rc = row_parallel(e->hbuf, e->I, w.wdown, w.wdown8, w.sdown, next_norm))) return rc;
   }
   B200_REQUIRE(e->ar_index == 0 || e->ar_index == 2 * e->L, "peer all-reduce count per step must be 2 per layer");
   if (nv == 2) {
@@ -664,6 +697,8 @@ static int graph_step(b200_engine* e, int key, Enqueue&& enqueue) {
   static const bool pf_on = getenv("B200_PREFETCHER") != nullptr;
   auto it = e->graphs.find(key);
   if (it == e->graphs.end()) {
+    // (the prefetch walk requests 16 KB bf16 weight tiles)
+    B200_REQUIRE(!(pf_on && e->fp8), "B200_PREFETCHER=1 is not supported with FP8 weights (weight_format 1)");
     const int before = e->launches;
     e->pf.active = pf_on; e->pf.recording = pf_on; e->pf.count = 0; e->pf.table.clear(); e->pf_cur = nullptr;
     int rc = enqueue();
@@ -1212,6 +1247,17 @@ static int cb_admit(b200_engine* e, int n, const int64_t* const* rows, const int
 }
 
 // shard copy helpers -------------------------------------------------------------------------------
+// the seven projection weights that weight_format 1 stores as e4m3 codes
+static bool is_fp8_projection(const std::string& rest) {
+  static const char* names[] = {"self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight",
+                                "self_attn.o_proj.weight", "mlp.gate_proj.weight", "mlp.up_proj.weight", "mlp.down_proj.weight"};
+  for (const char* x : names) if (rest == x) return true;
+  return false;
+}
+static int copy_2d(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t rows, bool on_device) {
+  B200_CUDA_OK(cudaMemcpy2D(dst, dpitch, src, spitch, width, rows, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+  return 0;
+}
 static int copy_rows(bf16* dst, const bf16* src, long long row0, long long rows, long long cols, bool on_device) {
   B200_CUDA_OK(cudaMemcpy(dst, src + row0 * cols, (size_t)rows * cols * 2, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
   return 0;
@@ -1252,6 +1298,9 @@ int b200_engine_create(const b200_model_config_t* c, const void* nccl_id, b200_e
   // over the running sequences when more than 64 are live.
   B200_REQUIRE(c->max_batch >= 1 && c->max_batch <= 512, "max_batch must be in [1, 512]");
   B200_REQUIRE(c->num_heads % c->num_kv_heads == 0 && c->num_heads / c->num_kv_heads <= 8, "GQA group must be <= 8");
+  B200_REQUIRE(c->weight_format == 0 || c->weight_format == 1, "weight_format must be 0 (bf16) or 1 (fp8 e4m3, a scale per row)");
+  B200_REQUIRE(c->weight_format == 0 || c->num_experts == 0, "FP8 weights are supported for dense models only (no MoE experts)");
+  B200_REQUIRE(c->weight_format == 0 || c->tp_size == 1, "FP8 weights are supported on one GPU only (tensor parallel tp_size > 1 is not)");
   int ndev = 0;
   B200_CUDA_OK(cudaGetDeviceCount(&ndev));
   B200_REQUIRE(c->device >= 0 && c->device < ndev, "no such CUDA device (this library has no CPU fallback)");
@@ -1294,13 +1343,25 @@ int b200_engine_create(const b200_model_config_t* c, const void* nccl_id, b200_e
   if ((rc = dmalloc(&e->lm_head, (size_t)e->Vl * H))) return rc;
   if ((rc = dmalloc(&e->final_norm, H))) return rc;
   e->layers.resize(e->L);
+  e->fp8 = c->weight_format == 1;
   for (auto& w : e->layers) {
-    if ((rc = dmalloc(&w.wqkv, (size_t)e->qkv_cols * H))) return rc;
-    if ((rc = dmalloc(&w.wo, H * e->nh * kHeadDim))) return rc;
-    if (e->E == 0) {
+    if (e->fp8) {
+      if ((rc = dmalloc(&w.wqkv8, (size_t)e->qkv_cols * H))) return rc;
+      if ((rc = dmalloc(&w.wo8, H * e->nh * kHeadDim))) return rc;
+      if ((rc = dmalloc(&w.wgu8, (size_t)2 * e->I * H))) return rc;
+      if ((rc = dmalloc(&w.wdown8, H * e->I))) return rc;
+      if ((rc = dmalloc(&w.sqkv, (size_t)e->qkv_cols))) return rc;
+      if ((rc = dmalloc(&w.so, H))) return rc;
+      if ((rc = dmalloc(&w.sgu, (size_t)2 * e->I))) return rc;
+      if ((rc = dmalloc(&w.sdown, H))) return rc;
+    } else {
+      if ((rc = dmalloc(&w.wqkv, (size_t)e->qkv_cols * H))) return rc;
+      if ((rc = dmalloc(&w.wo, H * e->nh * kHeadDim))) return rc;
+    }
+    if (e->E == 0 && !e->fp8) {
       if ((rc = dmalloc(&w.wgu, (size_t)2 * e->I * H))) return rc;
       if ((rc = dmalloc(&w.wdown, H * e->I))) return rc;
-    } else {
+    } else if (e->E > 0) {
       if ((rc = dmalloc(&w.wr, (size_t)e->E * H))) return rc;
       if ((rc = dmalloc(&w.wgu_e, (size_t)e->E * 2 * e->I * H))) return rc;
       if ((rc = dmalloc(&w.wdown_e, (size_t)e->E * H * e->I))) return rc;
@@ -1308,6 +1369,7 @@ int b200_engine_create(const b200_model_config_t* c, const void* nccl_id, b200_e
     if ((rc = dmalloc(&w.ln1, H))) return rc;
     if ((rc = dmalloc(&w.ln2, H))) return rc;
   }
+  if (e->fp8 && (rc = dmalloc(&e->wdq, (size_t)e->qkv_cols * H + H * e->nh * kHeadDim + (size_t)3 * e->I * H))) return rc;
   // rope tables (engine default: double-precision angles; hosts that need bit parity with
   // LlamaRotaryEmbedding pass their own via b200_engine_set_rope_table)
   {
@@ -1464,9 +1526,11 @@ int b200_engine_destroy(b200_engine_t* e) {
                   e->d_forced, e->d_eos, e->d_stop_tok, e->d_stop_off, e->d_state};
   for (void* p : ptrs) if (p) cudaFree(p);
   for (auto& w : e->layers) {
-    void* lp[] = {w.wqkv, w.wo, w.wgu, w.wdown, w.ln1, w.ln2, w.wr, w.wgu_e, w.wdown_e, w.bqkv};
+    void* lp[] = {w.wqkv, w.wo, w.wgu, w.wdown, w.ln1, w.ln2, w.wr, w.wgu_e, w.wdown_e, w.bqkv,
+                  w.wqkv8, w.wo8, w.wgu8, w.wdown8, w.sqkv, w.so, w.sgu, w.sdown};
     for (void* p : lp) if (p) cudaFree(p);
   }
+  if (e->wdq) cudaFree(e->wdq);
   for (auto& kv : e->host_kv) cudaFreeHost(kv.second);
   if (e->h_stage) cudaFreeHost(e->h_stage);
   if (e->h_state) cudaFreeHost(e->h_state);
@@ -1517,6 +1581,8 @@ int b200_engine_set_weight(b200_engine_t* e, const char* name, const void* data,
     const long long QH = (long long)e->cfg.num_heads * kHeadDim, KH = (long long)e->cfg.num_kv_heads * kHeadDim;
     const long long ql = (long long)e->nh * kHeadDim, kl = (long long)e->nkv * kHeadDim;
     const long long If = e->cfg.intermediate_size, Il = e->I;
+    B200_REQUIRE(!e->fp8 || !is_fp8_projection(rest),
+                 "this engine holds FP8 projection weights (weight_format 1): pass " + n + " to b200_engine_set_weight_fp8");
     if (rest == "input_layernorm.weight") {
       B200_REQUIRE(expect(H, -1), "shape mismatch for " + n);
       rc = copy_rows(w.ln1, src, 0, 1, H, dev);
@@ -1579,6 +1645,60 @@ int b200_engine_set_weight(b200_engine_t* e, const char* name, const void* data,
     return -5;
   }
   if (rc) return rc;
+  e->seen[n] = 1;
+  return 0;
+}
+
+int b200_engine_set_weight_fp8(b200_engine_t* e, const char* name, const void* data, const void* scale, int scale_dtype,
+                               int on_device, int ndim, const int64_t* shape) {
+  B200_REQUIRE(e && name && data && scale && shape, "null argument");
+  B200_REQUIRE(e->fp8, std::string("FP8 weight ") + name + " given to an engine created with weight_format 0 (bf16)");
+  B200_REQUIRE(scale_dtype == 0 || scale_dtype == 1, "scale_dtype must be 0 (bf16) or 1 (fp32)");
+  B200_CUDA_OK(cudaSetDevice(e->cfg.device));
+  const std::string n(name);
+  const bool dev = on_device != 0;
+  const size_t dot = n.rfind("model.layers.", 0) == 0 ? n.find('.', 13) : std::string::npos;
+  B200_REQUIRE(dot != std::string::npos && is_fp8_projection(n.substr(dot + 1)),
+               "FP8 weights are the q/k/v/o and gate/up/down projections only, got " + n);
+  const int l = atoi(n.substr(13, dot - 13).c_str());
+  B200_REQUIRE(l >= 0 && l < e->L, "layer index out of range in " + n);
+  const std::string rest = n.substr(dot + 1);
+  LayerW& w = e->layers[l];
+  const long long H = e->H;
+  const int r = e->cfg.tp_rank;
+  const long long QH = (long long)e->cfg.num_heads * kHeadDim, KH = (long long)e->cfg.num_kv_heads * kHeadDim;
+  const long long ql = (long long)e->nh * kHeadDim, kl = (long long)e->nkv * kHeadDim;
+  const long long If = e->cfg.intermediate_size, Il = e->I;
+  const char p0 = rest[0] == 's' ? rest[10] : rest[4];   // q / k / v / o, g(ate) / u(p) / d(own)
+  const long long rows = (p0 == 'q') ? QH : (p0 == 'k' || p0 == 'v') ? KH : (p0 == 'o' || p0 == 'd') ? H : If;
+  const long long cols = (p0 == 'o') ? QH : (p0 == 'd') ? If : H;
+  B200_REQUIRE(ndim == 2 && shape[0] == rows && shape[1] == cols, "shape mismatch for " + n);
+  // the scale of every row, as bf16: an fp32 scale is rounded to bf16 as transformers does when it loads the scale
+  // parameter into a bf16 model (W' = bf16(code) * bf16(scale) in bf16 arithmetic)
+  std::vector<bf16> hs((size_t)rows);
+  if (scale_dtype == 0) {
+    B200_CUDA_OK(cudaMemcpy(hs.data(), scale, rows * 2, dev ? cudaMemcpyDeviceToHost : cudaMemcpyHostToHost));
+  } else {
+    std::vector<float> f((size_t)rows);
+    B200_CUDA_OK(cudaMemcpy(f.data(), scale, rows * 4, dev ? cudaMemcpyDeviceToHost : cudaMemcpyHostToHost));
+    for (long long i = 0; i < rows; ++i) hs[i] = __float2bfloat16_rn(f[i]);
+  }
+  const uint8_t* src = reinterpret_cast<const uint8_t*>(data);
+  int rc = 0;
+  if (p0 == 'q' || p0 == 'k' || p0 == 'v') {   // column parallel: rows sharded, scales with their rows
+    const long long len = p0 == 'q' ? ql : kl, off = p0 == 'q' ? 0 : (p0 == 'k' ? ql : ql + kl);
+    if ((rc = copy_2d(w.wqkv8 + off * H, H, src + r * len * H, H, H, len, dev))) return rc;
+    B200_CUDA_OK(cudaMemcpy(w.sqkv + off, hs.data() + r * len, len * 2, cudaMemcpyHostToDevice));
+  } else if (p0 == 'g' || p0 == 'u') {          // 16-row gate / up interleave of this rank's rows, scales alike
+    const long long o16 = p0 == 'u' ? 16 : 0;
+    if ((rc = copy_2d(w.wgu8 + o16 * H, 32 * H, src + r * Il * H, 16 * H, 16 * H, Il / 16, dev))) return rc;
+    if ((rc = copy_2d(w.sgu + o16, 32 * 2, hs.data() + r * Il, 16 * 2, 16 * 2, Il / 16, false))) return rc;
+  } else {                                      // row parallel (o, down): columns sharded, every row's scale kept
+    const long long kf = p0 == 'o' ? QH : If, kloc = p0 == 'o' ? ql : Il;
+    uint8_t* dst = p0 == 'o' ? w.wo8 : w.wdown8;
+    if ((rc = copy_2d(dst, kloc, src + r * kloc, kf, kloc, H, dev))) return rc;
+    B200_CUDA_OK(cudaMemcpy(p0 == 'o' ? w.so : w.sdown, hs.data(), H * 2, cudaMemcpyHostToDevice));
+  }
   e->seen[n] = 1;
   return 0;
 }
@@ -2162,13 +2282,16 @@ static int op_sms() {
 }
 
 static int op_gemm(const void* A, const void* B, void* out, const void* residual, const void* bias, int M, int N, int K,
-                   int epi, int block_n, int splits, int64_t ldo, void* stream) {
+                   int epi, int block_n, int splits, int64_t ldo, void* stream, const void* a8 = nullptr,
+                   const void* a_scale = nullptr) {
   g_op_tmaps.maps.clear();  // caller buffers may be reused at other shapes
+  g_op_tmaps.maps_u8.clear();
   const bool t = epi >= EPI_T_STORE;
   int out_cols = (epi == EPI_SWIGLU) ? N / 2 : (epi == EPI_T_SWIGLU ? M / 2 : 0);
   GemmArgs a{(const bf16*)A, M, (const bf16*)B, N, M, N, K, epi, block_n, effective_splits(K, splits), out,
              (const bf16*)residual, ldo, (long long)N * ldo, out_cols, t};
   a.bias = (const bf16*)bias;
+  a.a8 = (const uint8_t*)a8; a.a_scale = (const bf16*)a_scale;
   static float* op_sk_ws = nullptr;
   static int* op_sk_flags = nullptr;
   const int op_sk_tiles = 2048;
@@ -2190,6 +2313,23 @@ int b200_op_gemm_bias(const void* A, const void* B, void* out, const void* resid
                       int block_n, int splits, int64_t ldo, const void* bias, void* stream) {
   B200_REQUIRE(bias != nullptr && (epi == EPI_STORE || epi == EPI_T_STORE), "b200_op_gemm_bias: a bias with epi 0 or 3");
   return op_gemm(A, B, out, residual, bias, M, N, K, epi, block_n, splits, ldo, stream);
+}
+
+int b200_op_gemm_fp8(const void* A8, const void* scale, const void* B, void* out, const void* bias, int M, int N, int K,
+                     int epi, int block_n, int splits, int64_t ldo, void* stream) {
+  B200_REQUIRE(A8 && scale && epi >= EPI_T_STORE && epi <= EPI_T_PARTIAL, "b200_op_gemm_fp8: FP8 weights, a scale per row, epi 3-5");
+  B200_REQUIRE(!bias || epi == EPI_T_STORE, "b200_op_gemm_fp8: a bias needs epi 3");
+  return op_gemm(nullptr, B, out, nullptr, bias, M, N, K, epi, block_n, splits, ldo, stream, A8, scale);
+}
+
+int b200_op_dequant_fp8(const void* q, const void* scale, void* out, int64_t rows, int K, void* stream) {
+  B200_REQUIRE(q && scale && out && rows >= 0 && K % 16 == 0, "b200_op_dequant_fp8: K must be a multiple of 16");
+  B200_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
+               "b200_op_dequant_fp8: 16-byte aligned buffers");
+  Fp8Segs sg{};
+  sg.seg[0] = Fp8Seg{(const uint8_t*)q, (const bf16*)scale, (bf16*)out, rows * K / 16, K};
+  sg.n = 1;
+  return launch_dequant_fp8(sg, (cudaStream_t)stream);
 }
 
 int b200_op_rmsnorm(void* x, const void* w, void* xn, int rows, int H, float eps, const float* partial, int splits,

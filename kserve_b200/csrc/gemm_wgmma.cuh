@@ -72,6 +72,8 @@ struct GemmParams {
   // per-output-feature bias (EPI_STORE, EPI_ROPE_KV: column n; EPI_T_STORE: weight row m), nullptr = none.  It is added
   // in fp32 to the finished accumulator, so the output is ONE bf16 rounding of (acc + bias) as nn.Linear(bias=True) gives.
   const bf16* bias;
+  // FP8 weights (gemm_tn_kernel<..., true>): A is e4m3 [M][K] and a_scale[m] the bf16 scale of weight row m
+  const bf16* a_scale;
 };
 
 constexpr int kGemmBlockM = 128;
@@ -80,18 +82,22 @@ constexpr int kGemmThreads = 384;
 constexpr int kGemmGroupM = 16;
 constexpr int kStgStride = 132;   // floats between two staged accumulator columns: 128 rows + 4 (conflict-free fragment stores)
 
-template <int BLOCK_N>
+template <int BLOCK_N, bool FP8A = false>
 struct GemmCfg {
   static_assert(BLOCK_N <= 64, "swap-AB tiles carry the batch in N");
-  static constexpr int kABytes = kGemmBlockM * kGemmBlockK * 2;  // 16 KB
+  static constexpr int kABytes = kGemmBlockM * kGemmBlockK * (FP8A ? 1 : 2);  // 16 KB (8 KB of e4m3 codes)
   static constexpr int kBBytes = BLOCK_N * kGemmBlockK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = 8;
+  // FP8: every consumer warpgroup expands its 64-row half of the A tile into one of 3 bf16 buffers (8 KB each) that
+  // wgmma reads; 3 because the k-block before the previous one may still be in flight when the next one is written
+  static constexpr int kXBufs = FP8A ? 3 : 0;
+  static constexpr int kXBytes = 2 * kXBufs * 64 * kGemmBlockK * 2;
   static constexpr int kChunk = (BLOCK_N >= 32) ? 32 : 16;             // columns one epilogue thread takes at a time
   static constexpr int kRoundCols = BLOCK_N;                           // columns staged per epilogue round
   static constexpr int kChunks = kRoundCols / kChunk;
   static constexpr int kStgBytes = kRoundCols * kStgStride * 4;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kStgBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kXBytes + kStgBytes + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(kSmemBytes <= 227 * 1024, "GEMM shared memory exceeds the 227 KB a block may use");
 };
 
@@ -116,6 +122,72 @@ __device__ __forceinline__ void st_out_v4(bf16* p, const uint4& o, int stream_ou
 // (rel. error ~1e-6) cannot change the bf16 result except on exact rounding ties, and keep the epilogue short.
 __device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 
+
+// ---- FP8 (e4m3) weights
+// The engine multiplies exactly the bf16 operand compressed-tensors' decompression gives transformers:
+// W' = bf16(code) * s in bf16 arithmetic (one round-to-nearest-even), s = the row's scale rounded to bf16.
+// e4m3 -> bf16 is exact: the code's 7 exponent / mantissa bits are moved to their bf16 position, which gives a bf16 of
+// 2^-120 times the code's value (subnormal codes become bf16 subnormals), and multiplied back by 2^120 (exact).
+// The NaN codes 0x7F / 0xFF would come out as +-480 * s: the loader refuses checkpoints that contain them.
+__device__ __forceinline__ uint32_t bf16x2_mul(uint32_t a, uint32_t b) {
+  uint32_t d;
+  asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
+  return d;
+}
+// A row's scale as the pair the expansion multiplies by: {s * 2^120, s * 2^120} when |s| < 2^8 (exact and finite, and
+// then ONE multiply gives bf16(code * s) with a single rounding), else {s, s} after an exact multiply by 2^120
+struct Fp8Scale { uint32_t s2; bool folded; };
+__device__ __forceinline__ uint32_t bf16_pair(bf16 s) {
+  const uint32_t u = *reinterpret_cast<const unsigned short*>(&s);
+  return u | (u << 16);
+}
+__device__ __forceinline__ Fp8Scale fp8_scale(bf16 s) {
+  const float f = __bfloat162float(s);
+  const bool folded = fabsf(f) < 256.f;
+  return Fp8Scale{bf16_pair(folded ? __float2bfloat16_rn(f * 0x1p120f) : s), folded};
+}
+// 4 codes of `w` (byte order) -> bf16 pairs {code0, code1} in lo, {code2, code3} in hi, each times the row's scale
+__device__ __forceinline__ void fp8x4_dequant(uint32_t w, const Fp8Scale& sc, uint32_t& lo, uint32_t& hi) {
+  constexpr uint32_t kPow120 = 0x7B807B80u;   // {2^120, 2^120}
+  const uint32_t a = __byte_perm(w, 0, 0x1404), b = __byte_perm(w, 0, 0x3424);   // each code in the high byte of a half
+  lo = (a & 0x80008000u) | ((a >> 4) & 0x07F007F0u);
+  hi = (b & 0x80008000u) | ((b >> 4) & 0x07F007F0u);
+  if (!sc.folded) {
+    lo = bf16x2_mul(lo, kPow120);
+    hi = bf16x2_mul(hi, kPow120);
+  }
+  lo = bf16x2_mul(lo, sc.s2);
+  hi = bf16x2_mul(hi, sc.s2);
+}
+// 16 codes -> 16 bf16 (two 16-byte chunks)
+__device__ __forceinline__ void fp8x16_dequant(const uint4& v, const Fp8Scale& sc, uint4& o0, uint4& o1) {
+  fp8x4_dequant(v.x, sc, o0.x, o0.y);
+  fp8x4_dequant(v.y, sc, o0.z, o0.w);
+  fp8x4_dequant(v.z, sc, o1.x, o1.y);
+  fp8x4_dequant(v.w, sc, o1.z, o1.w);
+}
+
+// A layer's FP8 matrices -> bf16 (prefill feeds the unchanged bf16 GEMM from this scratch); K % 16 == 0
+struct Fp8Seg { const uint8_t* q; const bf16* s; bf16* out; long long chunks; int K; };   // chunks = rows * K / 16
+struct Fp8Segs { Fp8Seg seg[4]; int n; };
+
+__global__ void __launch_bounds__(256) dequant_fp8_kernel(const Fp8Segs p) {
+  long long total = 0;
+  for (int i = 0; i < p.n; ++i) total += p.seg[i].chunks;
+  for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < total; c += (long long)gridDim.x * blockDim.x) {
+    long long cc = c;
+    int i = 0;
+    while (cc >= p.seg[i].chunks) { cc -= p.seg[i].chunks; ++i; }
+    const Fp8Seg& g = p.seg[i];
+    const long long row = cc * 16 / g.K;
+    const uint4 v = ld_nc_v4(g.q + cc * 16);
+    uint4 o0, o1;
+    fp8x16_dequant(v, fp8_scale(g.s[row]), o0, o1);
+    uint4* o = reinterpret_cast<uint4*>(g.out + cc * 16);
+    o[0] = o0;
+    o[1] = o1;
+  }
+}
 
 struct GemmSeg { int m_t, n_t, kb0, kb1, split, type, slot; };  // type: 0 full tile, 1 partial piece -> workspace slot, 2 tile-finishing piece (adds `slot` parked pieces)
 
@@ -182,19 +254,23 @@ __device__ __forceinline__ bool gemm_get_seg(const GemmParams& p, int idx, GemmS
   return gemm_get_seg(sc, idx, g, m_tiles_rt, (int)blockIdx.x, (int)gridDim.x);
 }
 
-template <int BLOCK_N, int EPI>
+// FP8A: A is e4m3 (weights with a bf16 scale per row, p.a_scale); the consumers expand every k-block's A tile into the
+// bf16 layout the bf16 kernel's TMA would have written (128B swizzle), so the MMAs, their k order, the schedule and the
+// epilogues are those of the bf16 kernel on W' (bit-identical results), while HBM streams one byte per weight.
+template <int BLOCK_N, int EPI, bool FP8A = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const GemmParams p) {
   static_assert(EPI == EPI_T_STORE || EPI == EPI_T_SWIGLU || EPI == EPI_T_PARTIAL, "swap-AB epilogues only");
   TraceScope _ts(TK_GEMM + 100 * EPI + 1000 * (p.M >> 7));
-  using Cfg = GemmCfg<BLOCK_N>;
+  using Cfg = GemmCfg<BLOCK_N, FP8A>;
   constexpr int STAGES = Cfg::kStages;
   constexpr int CH = Cfg::kChunk;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* stg = reinterpret_cast<float*>(smem + STAGES * Cfg::kStageBytes);   // [kRoundCols][kStgStride] fp32
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::kStageBytes + Cfg::kStgBytes);
+  uint8_t* xbuf = smem + STAGES * Cfg::kStageBytes;   // FP8A: [2 warpgroups][kXBufs][64 rows][128 B] bf16, swizzled
+  float* stg = reinterpret_cast<float*>(xbuf + Cfg::kXBytes);   // [kRoundCols][kStgStride] fp32
+  uint64_t* bars = reinterpret_cast<uint64_t*>(xbuf + Cfg::kXBytes + Cfg::kStgBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
 
@@ -289,6 +365,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     int stage = 0;
     uint32_t phase = 0;
     float accum[BLOCK_N / 2];
+    int xk = 0;               // FP8A: k-blocks expanded so far (selects the bf16 buffer)
     GemmSeg sg;
     for (int idx = 0; gemm_get_seg(p, idx, sg, m_tiles_rt); ++idx) {
       const int n_t = sg.n_t, s = sg.split, kb0 = sg.kb0, kb1 = sg.kb1;
@@ -302,13 +379,41 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         m_t -= g * gmt;         // tile index inside the group: output features are per expert
         out_off = (long long)g * p.group_out_stride;
       }
+      // FP8A: this thread expands two 16-byte chunks of codes per k-block, rows t/4 and t/4 + 32 of the warpgroup's half
+      Fp8Scale xsc[2] = {{0u, true}, {0u, true}};
+      if constexpr (FP8A) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int row = m_t * kGemmBlockM + half * 64 + (t >> 2) + 32 * i;
+          if (row < p.M) xsc[i] = fp8_scale(p.a_scale[row]);   // (rows past M: TMA zero-filled codes, scale 0)
+        }
+      }
       // ---- main loop: one k-block in flight behind the one being issued
       wgmma_keep(accum);
       int prev = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-        const uint64_t adesc = make_smem_desc_sw128(sa + half * 64 * 128);
+        uint64_t adesc;
+        if constexpr (FP8A) {
+          // codes: [128 rows][64 B] unswizzled; bf16: [64 rows][128 B], 16-byte chunk c of row r at chunk c ^ (r & 7)
+          const uint8_t* a8 = smem + stage * Cfg::kStageBytes + half * 64 * kGemmBlockK;
+          uint8_t* xb = xbuf + (half * Cfg::kXBufs + xk % Cfg::kXBufs) * (64 * 128);
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const int j = t + 128 * i, r = j >> 2, c0 = (j & 3) * 2;
+            uint4 o0, o1;
+            fp8x16_dequant(*reinterpret_cast<const uint4*>(a8 + j * 16), xsc[i], o0, o1);
+            *reinterpret_cast<uint4*>(xb + r * 128 + ((c0 ^ (r & 7)) << 4)) = o0;
+            *reinterpret_cast<uint4*>(xb + r * 128 + (((c0 + 1) ^ (r & 7)) << 4)) = o1;
+          }
+          fence_proxy_async_shared();   // generic-proxy stores -> visible to wgmma
+          asm volatile("bar.sync %0, 128;" ::"r"(2 + half) : "memory");
+          adesc = make_smem_desc_sw128(smem_u32(xb));
+          ++xk;
+        } else {
+          adesc = make_smem_desc_sw128(sa + half * 64 * 128);
+        }
         const uint64_t bdesc = make_smem_desc_sw128(sa + Cfg::kABytes);
         wgmma_fence();
 #pragma unroll

@@ -59,8 +59,37 @@ inline int make_tmap_2d(CUtensorMap* map, const void* ptr, uint64_t rows, uint64
   return 0;
 }
 
+// 2D e4m3 codes [rows][cols] (FP8 weights), box = [box_rows][64 bytes], unswizzled, OOB -> zeros.
+inline int make_tmap_2d_u8(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+  PFN_encodeTiled fn = get_encode_fn();
+  B200_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled entry point not available (no CUDA driver?)");
+  B200_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && cols % 16 == 0, "FP8 TMA: 16-byte aligned base and rows");
+  cuuint64_t dims[2] = {cols, rows};
+  cuuint64_t strides[1] = {cols};
+  cuuint32_t box[2] = {64, box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  B200_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (u8) failed with CUresult " + std::to_string((int)r));
+  return 0;
+}
+
 struct TmapCache {
   std::map<std::tuple<const void*, uint64_t, uint64_t, uint32_t, uint64_t>, CUtensorMap> maps;
+  std::map<std::tuple<const void*, uint64_t, uint64_t>, CUtensorMap> maps_u8;   // FP8 weights, 128-row boxes
+  int get_u8(const void* ptr, uint64_t rows, uint64_t cols, const CUtensorMap** out) {
+    auto key = std::make_tuple(ptr, rows, cols);
+    auto it = maps_u8.find(key);
+    if (it == maps_u8.end()) {
+      CUtensorMap m;
+      int rc = make_tmap_2d_u8(&m, ptr, rows, cols, 128);
+      if (rc) return rc;
+      it = maps_u8.emplace(key, m).first;
+    }
+    *out = &it->second;
+    return 0;
+  }
   // ld_elems: row pitch in elements, 0 = dense rows (cols)
   int get(const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows, const CUtensorMap** out, uint64_t ld_elems = 0) {
     if (ld_elems == 0) ld_elems = cols;
@@ -121,15 +150,26 @@ int launch_prefill_inst(const CUtensorMap* ta, const CUtensorMap* tb, const CUte
   return 0;
 }
 
-template <int BLOCK_N, int EPI>
+template <int BLOCK_N, int EPI, bool FP8A = false>
 int launch_gemm_inst(const CUtensorMap* ta, const CUtensorMap* tb, const GemmParams& p, int grid, cudaStream_t s) {
-  auto kern = gemm_tn_kernel<BLOCK_N, EPI>;
+  auto kern = gemm_tn_kernel<BLOCK_N, EPI, FP8A>;
+  constexpr int smem = GemmCfg<BLOCK_N, FP8A>::kSmemBytes;
   static bool configured = false;  // per instantiation
   if (!configured) {
-    B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<BLOCK_N>::kSmemBytes));
+    B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = true;
   }
-  B200_CUDA_OK(launch_k(kern, dim3(grid), dim3(kGemmThreads), GemmCfg<BLOCK_N>::kSmemBytes, s, *ta, *tb, p));
+  B200_CUDA_OK(launch_k(kern, dim3(grid), dim3(kGemmThreads), smem, s, *ta, *tb, p));
+  return 0;
+}
+
+// a layer's FP8 matrices -> bf16 (prefill), one launch
+inline int launch_dequant_fp8(const Fp8Segs& segs, cudaStream_t s) {
+  long long total = 0;
+  for (int i = 0; i < segs.n; ++i) total += segs.seg[i].chunks;
+  if (total == 0) return 0;
+  const int grid = (int)std::min<long long>((total + 255) / 256, 132 * 16);
+  B200_CUDA_OK(launch_k(dequant_fp8_kernel, dim3(grid), dim3(256), 0, s, segs));
   return 0;
 }
 
@@ -162,6 +202,8 @@ struct GemmArgs {
   PfCtx* pf = nullptr;              // weight-stream prefetcher context of the step being enqueued (decode only)
   const RopeKvParams* rope = nullptr;   // EPI_ROPE_KV: where RoPE(k) / v go and the tables (q is rotated in place in `out`)
   const bf16* bias = nullptr;       // per-output-feature bias (EPI_STORE, EPI_ROPE_KV, EPI_T_STORE), see GemmParams::bias
+  const uint8_t* a8 = nullptr;      // FP8 weights: e4m3 A [a_rows][K] replacing `A`, with a bf16 scale per row (swap-AB only)
+  const bf16* a_scale = nullptr;
 };
 
 // GEMMs whose weight operand depends on nothing the step computes (decode swap-AB, no device-side extents)
@@ -170,7 +212,14 @@ inline bool pf_eligible(const GemmArgs& a) { return a.stream_a && !a.n_rt && !a.
 inline int launch_gemm(TmapCache& cache, const GemmArgs& a, int num_sms, cudaStream_t s) {
   B200_REQUIRE(a.K % 8 == 0, "K must be a multiple of 8");
   const CUtensorMap *ta, *tb;
-  int rc = cache.get(a.A, a.a_rows, a.K, kGemmBlockM, &ta);
+  int rc;
+  if (a.a8) {
+    B200_REQUIRE(a.stream_a && a.a_scale && a.groups == 0 && !a.m_rt && !a.n_rt && !a.row_off && a.K % 16 == 0,
+                 "FP8 weights: an ungrouped swap-AB GEMM with a scale per weight row and K a multiple of 16");
+    rc = cache.get_u8(a.a8, a.a_rows, a.K, &ta);
+  } else {
+    rc = cache.get(a.A, a.a_rows, a.K, kGemmBlockM, &ta);
+  }
   if (rc) return rc;
   rc = cache.get(a.B, a.b_rows, a.K, a.block_n, &tb);
   if (rc) return rc;
@@ -217,7 +266,7 @@ inline int launch_gemm(TmapCache& cache, const GemmArgs& a, int num_sms, cudaStr
       p.sched = 1; p.sk_slots = slots; grid = g2;
     }
   }
-  if (a.pf && a.pf->active && pf_eligible(a) && p.n_tiles == 1) {
+  if (a.pf && a.pf->active && pf_eligible(a) && p.n_tiles == 1 && !a.a8) {
     if (a.pf->recording && a.pf->count < kPfMaxGemms) {
       PfGemm g{};
       g.tmap_a = *ta;
@@ -231,6 +280,7 @@ inline int launch_gemm(TmapCache& cache, const GemmArgs& a, int num_sms, cudaStr
   B200_REQUIRE(!a.bias || ((a.epi == EPI_STORE || a.epi == EPI_ROPE_KV || a.epi == EPI_T_STORE) && a.groups == 0),
                "a GEMM bias needs the EPI_STORE, EPI_ROPE_KV or EPI_T_STORE epilogue of an ungrouped GEMM");
   p.bias = a.bias;
+  p.a_scale = a.a_scale;
   p.rope_tok_seq = nullptr; p.rope_tok_pos = nullptr; p.rope_page_table = nullptr; p.rope_max_pages = 0;
   p.rope_kcache = nullptr; p.rope_vcache = nullptr; p.rope_cos = nullptr; p.rope_sin = nullptr; p.rope_nh = 0; p.rope_nkv = 0;
   if (a.epi == EPI_ROPE_KV) {
@@ -260,8 +310,9 @@ inline int launch_gemm(TmapCache& cache, const GemmArgs& a, int num_sms, cudaStr
     return a.bias ? launch_prefill_inst<EPI_ROPE_KV, true>(ta, tb, to, p, grid, s)
                   : launch_prefill_inst<EPI_ROPE_KV>(ta, tb, to, p, grid, s);
   }
-#define B200_GEMM_CASE(BN, E) \
-  if (a.block_n == BN && a.epi == E) return launch_gemm_inst<BN, E>(ta, tb, p, grid, s);
+#define B200_GEMM_CASE(BN, E)                                                                             \
+  if (a.block_n == BN && a.epi == E)                                                                      \
+    return a.a8 ? launch_gemm_inst<BN, E, true>(ta, tb, p, grid, s) : launch_gemm_inst<BN, E>(ta, tb, p, grid, s);
   B200_GEMM_CASE(16, EPI_T_STORE)
   B200_GEMM_CASE(16, EPI_T_SWIGLU)
   B200_GEMM_CASE(16, EPI_T_PARTIAL)

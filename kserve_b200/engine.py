@@ -43,7 +43,8 @@ class B200Engine:
     def __init__(self, cfg: dict, *, max_batch: int = 8, max_seq_len: int = 2048,
                  max_prefill_tokens: Optional[int] = None, num_kv_pages: int = 0, device: int = 0,
                  tp_rank: int = 0, tp_size: int = 1, nccl_id: Optional[bytes] = None,
-                 vocab_rows: Optional[int] = None):
+                 vocab_rows: Optional[int] = None, weight_format: int = 0):
+        """weight_format 1: the seven projection weights are FP8 (float8_e4m3fn + a scale per row, kserve_b200/fp8.py)"""
         self.lib = _lib.load()
         if not torch.cuda.is_available():
             raise _lib.B200Error("no CUDA device: kserve_b200 has no CPU fallback")
@@ -69,6 +70,8 @@ class B200Engine:
         mc.tp_rank, mc.tp_size, mc.device = tp_rank, tp_size, device
         mc.num_experts = int(cfg.get("num_local_experts", 0) or 0)
         mc.num_experts_per_tok = int(cfg.get("num_experts_per_tok", 0) or 0) if mc.num_experts else 0
+        mc.weight_format = int(weight_format)
+        self.weight_format = int(weight_format)
         self.device = device
         self.tp_size, self.tp_rank = tp_size, tp_rank
         # rope tables first: an unsupported rope_scaling type must fail before any device memory is taken
@@ -115,9 +118,41 @@ class B200Engine:
         _lib.check(self.lib.b200_engine_set_weight(self.h, name.encode(), t.data_ptr(), on_dev, t.dim(), shape),
                    f"set_weight({name})")
 
+    def set_weight_fp8(self, name: str, w: torch.Tensor, scale: torch.Tensor) -> None:
+        """an FP8 projection weight: e4m3 codes [out, in] and its checkpoint weight_scale (channel or tensor)"""
+        from .fp8 import row_scales
+        if w.dtype != torch.float8_e4m3fn:
+            raise _lib.B200Error(f"set_weight_fp8({name}): expected float8_e4m3fn codes, got {w.dtype}")
+        w = w.contiguous()
+        if bool(((w.view(torch.uint8) & 0x7F) == 0x7F).any()):
+            # (e4m3fn has no infinities; 0x7F / 0xFF are its NaNs, which no quantizer writes for a finite weight)
+            raise _lib.B200Error(f"set_weight_fp8({name}): the weight holds NaN codes")
+        s = row_scales(scale, w.shape[0]).to(w.device)
+        if s.dtype != torch.bfloat16:
+            s = s.to(torch.float32)             # (exact for fp16 / fp32; the engine rounds it to bf16 as transformers does)
+        s = s.contiguous()
+        shape = (C.c_int64 * 2)(*w.shape)
+        _lib.check(self.lib.b200_engine_set_weight_fp8(self.h, name.encode(), w.data_ptr(), s.data_ptr(),
+                                                       0 if s.dtype == torch.bfloat16 else 1, 1 if w.is_cuda else 0, 2, shape),
+                   f"set_weight_fp8({name})")
+
     def load_weights(self, named_tensors: Iterable[Tuple[str, torch.Tensor]]) -> None:
+        """HF state_dict tensors; FP8 `<proj>.weight` codes are paired with their `<proj>.weight_scale` in any order"""
+        pending = {}
         for name, t in named_tensors:
+            if name.endswith(".input_scale"):
+                raise _lib.B200Error(f"{name}: static FP8 activation scales are not supported (activations stay bf16)")
+            if name.endswith(".weight_scale") or (name.endswith(".weight") and t.dtype == torch.float8_e4m3fn):
+                base = name[:-len("_scale")] if name.endswith("_scale") else name
+                pair = pending.setdefault(base, {})
+                pair["scale" if name.endswith("_scale") else "w"] = t
+                if len(pair) == 2:
+                    self.set_weight_fp8(base, pair["w"], pair["scale"])
+                    del pending[base]
+                continue
             self.set_weight(name, t)
+        if pending:
+            raise _lib.B200Error("FP8 weights and scales must come in pairs; unpaired: " + ", ".join(sorted(pending)))
         _lib.check(self.lib.b200_engine_finalize_weights(self.h), "finalize_weights")
 
     # ------------------------------------------------------------------ generate

@@ -22,6 +22,7 @@ import numpy as np
 import torch
 
 from .engine import B200Engine, GenerateResult
+from .fp8 import UnsupportedQuantization, log_activation_scheme, parse_quantization_config
 from .utils import get_and_verify_max_len, logger, plan_memory, rope_inv_freq
 from .kserve_api.errors import InvalidInput
 from .kserve_api.metrics import DECODE_TOKENS_PER_S, LLM_STATS_KEY, TTFT_HIST, LLMStats, get_labels
@@ -195,6 +196,12 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
                 raise OpenAIError(f"config.{key}=true is not supported by the H100 runtime")
         if cfg.get("hidden_act", "silu") != "silu":
             raise OpenAIError(f"hidden_act={cfg.get('hidden_act')} is not supported by the H100 runtime (silu only)")
+        try:
+            quant = parse_quantization_config(cfg, self.tp_size)     # None = bf16 checkpoint; FP8: kserve_b200/fp8.py
+        except UnsupportedQuantization as e:
+            raise OpenAIError(str(e))
+        if quant is not None:
+            log_activation_scheme(quant)
         # checkpoint generation defaults: transformers merges the None fields of the request's GenerationConfig from
         # model.generation_config (generation/utils.py:1693-1701) — this is how instruct checkpoints turn sampling on (q9)
         self.generation_defaults = dict(self._generation_defaults or {})
@@ -224,7 +231,8 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
         self.max_prefill_tokens = cap_t
         self._engine = B200Engine(cfg, max_batch=self.max_batch, max_seq_len=self.max_length, device=self.device_index,
                                   max_prefill_tokens=cap_t, num_kv_pages=pages,
-                                  tp_rank=self.tp_rank, tp_size=self.tp_size, nccl_id=self.nccl_id, vocab_rows=vocab_rows)
+                                  tp_rank=self.tp_rank, tp_size=self.tp_size, nccl_id=self.nccl_id, vocab_rows=vocab_rows,
+                                  weight_format=0 if quant is None else 1)
         weights = self._state_dict if self._state_dict is not None else load_safetensors_dir(self.model_id_or_path)
         V0 = cfg["vocab_size"]
 

@@ -147,7 +147,8 @@ def plan_memory(cfg: Dict[str, Any], vocab_rows: int, max_batch: int, max_len: i
     The engine preallocates its activation buffers for `max_prefill_tokens` packed prompt tokens and a pool of 64-token
     KV pages; sizing both as max_batch x max_model_len (a Llama-3.1 config says 131072) would not fit any GPU, so the
     prefill buffers are capped (one full-length prompt always fits) and the page pool takes what is left, at most
-    max_batch full-length sequences and at least one."""
+    max_batch full-length sequences and at least one.  An FP8 checkpoint (kserve_b200/fp8.py) keeps one byte per
+    projection weight plus a bf16 scale per row, and a bf16 scratch of one layer's projections for prefill."""
     H, I, L = cfg["hidden_size"], cfg["intermediate_size"], cfg["num_hidden_layers"]
     nh, nkv = cfg["num_attention_heads"], cfg["num_key_value_heads"]
     d = cfg.get("head_dim") or H // nh
@@ -156,6 +157,11 @@ def plan_memory(cfg: Dict[str, Any], vocab_rows: int, max_batch: int, max_len: i
     qkv_cols = (nh_l + 2 * nkv_l) * d
     layer = qkv_cols * H + H * nh_l * d + (E * (3 * H * I_l) + E * H if E else 3 * H * I_l) + 2 * H
     weights = 2 * (L * layer + vocab_rows * H + -(-vocab_rows // tp_size) * H + H)
+    if cfg.get("quantization_config"):     # (validated by load(): an FP8 checkpoint, kserve_b200/fp8.py)
+        linear = qkv_cols * H + H * nh_l * d + 3 * H * I_l
+        scale_rows = qkv_cols + H + 2 * I_l + H
+        weights -= L * (2 * linear - (linear + 2 * scale_rows))
+        weights += 2 * linear
     per_tok = 2 * (3 * H + qkv_cols + nh_l * d + I_l) + 16 + (2 * (3 * H + 2 * I_l) + 24 if E else 0)
     page = L * 2 * nkv_l * 64 * d * 2
     pages_per_seq = -(-max_len // 64)

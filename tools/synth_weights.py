@@ -96,6 +96,41 @@ for _base in ("tiny_qwen2", "qwen2_7b_2l"):
     QWEN2_CONFIGS[_base + "_peaked"] = dict(QWEN2_CONFIGS[_base], _peaked=True)
 CONFIGS.update(QWEN2_CONFIGS)
 
+# FP8 checkpoints (compressed-tensors float-quantized, kserve_b200/fp8.py): the SAME seeded bf16 tensors as the base
+# config, each q/k/v/o/gate/up/down projection quantized to float8_e4m3fn with a scale amax / 448 per row ("channel") or
+# per tensor ("tensor"), in bf16 or fp32; everything else (embeddings, norms, lm_head, Qwen2 biases) stays bf16.
+# iter_state_dict yields `<proj>.weight` codes followed by `<proj>.weight_scale`, as such a checkpoint holds them.
+FP8_CONFIGS: Dict[str, dict] = {
+    "tiny_g4_fp8": dict(CONFIGS["tiny_g4"], _fp8="channel"),
+    "tiny_g4_fp8_peaked": dict(CONFIGS["tiny_g4_peaked"], _fp8="channel"),
+    "tiny_qwen2_fp8": dict(CONFIGS["tiny_qwen2"], _fp8="channel"),                               # biases, G = 7
+    "tiny_g2_fp8_tensor": dict(CONFIGS["tiny_g2"], _fp8="tensor", _fp8_scale="float32"),
+    "tiny_qwen2_g6_tied_fp8": dict(CONFIGS["tiny_qwen2_g6_tied"], _fp8="channel", _fp8_scale="float32"),
+    "llama3_8b_2l_fp8": dict(CONFIGS["llama3_8b_2l"], _fp8="channel"),
+    "llama3_8b_2l_fp8_peaked": dict(CONFIGS["llama3_8b_2l_peaked"], _fp8="channel"),
+}
+CONFIGS.update(FP8_CONFIGS)
+FP8_PROJECTIONS = ("self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight", "self_attn.o_proj.weight",
+                   "mlp.gate_proj.weight", "mlp.up_proj.weight", "mlp.down_proj.weight")
+
+
+def fp8_quantize(t: torch.Tensor, strategy: str = "channel", scale_dtype=torch.bfloat16):
+    """(e4m3 codes, weight_scale) of a weight: scale = amax / 448 ([out, 1] per row, [1] per tensor), codes = w / scale"""
+    t = t.float()
+    amax = t.abs().amax(dim=1, keepdim=True) if strategy == "channel" else t.abs().amax().reshape(1)
+    scale = (amax / 448.0).clamp_min(1e-12).to(scale_dtype)
+    codes = (t / (scale.float() if strategy == "channel" else scale.float()[0])).clamp(-448.0, 448.0)
+    return codes.to(torch.float8_e4m3fn), scale
+
+
+def fp8_quantization_config(strategy: str) -> dict:
+    """config.json's quantization_config of an FP8 config (what llm-compressor writes for weight-only FP8)"""
+    return dict(quant_method="compressed-tensors", format="float-quantized", quantization_status="compressed",
+                ignore=["lm_head"], kv_cache_scheme=None,
+                config_groups={"group_0": dict(targets=["Linear"], input_activations=None, output_activations=None,
+                                               weights=dict(num_bits=8, type="float", symmetric=True, strategy=strategy,
+                                                            dynamic=False))})
+
 
 def hf_config_dict(cfg: dict) -> dict:
     """the keys a transformers config understands (drops this module's private `_...` markers)"""
@@ -186,6 +221,17 @@ def peaked_perm(vocab: int, seed: int) -> torch.Tensor:
 
 def iter_state_dict(cfg: dict, seed: int = 0, dtype=torch.bfloat16):
     """Yield (name, tensor) one tensor at a time (bounded memory)."""
+    if cfg.get("_fp8"):
+        base = {k: v for k, v in cfg.items() if k not in ("_fp8", "_fp8_scale")}
+        sdt = getattr(torch, cfg.get("_fp8_scale", "bfloat16"))
+        for name, t in iter_state_dict(base, seed, dtype):
+            if name.split(".", 3)[-1] in FP8_PROJECTIONS:
+                codes, scale = fp8_quantize(t, cfg["_fp8"], sdt)
+                yield name, codes
+                yield name + "_scale", scale
+            else:
+                yield name, t
+        return
     for idx, (name, shape, kind) in enumerate(tensor_specs(cfg)):
         if name == "lm_head.weight" and cfg.get("_peaked"):
             embed = synth_tensor(0, shape, "embed", seed, dtype)      # index 0 == model.embed_tokens.weight
