@@ -207,10 +207,28 @@ int b200_op_attn_prefill_tc(const void* q, int64_t ldq, int q_rows, void* out, i
                             const void* vcache, int num_pages, const int32_t* page_table, int max_pages,
                             const int32_t* cu_seqlens, const int32_t* seq_slot, int B, int max_len, int nh, int nkv,
                             void* stream);
+/* b200_op_attn_prefill_tc for chunked prefill / prefix reuse: kv_off = device int32 [B], each a multiple of 128; the
+ * cu_seqlens rows of sequence b are its positions kv_off[b] ..., and its keys [0, kv_off[b]) are already in the cache */
+int b200_op_attn_prefill_tc_off(const void* q, int64_t ldq, int q_rows, void* out, int64_t ldo, const void* kcache,
+                                const void* vcache, int num_pages, const int32_t* page_table, int max_pages,
+                                const int32_t* cu_seqlens, const int32_t* seq_slot, const int32_t* kv_off, int B, int max_len,
+                                int nh, int nkv, void* stream);
+/* decode attention on already-roped queries (q [B][ldq]); splits > 1 merges with a separate combine kernel */
 int b200_op_attn_decode(const void* q, int64_t ldq, void* out, int64_t ldo, const void* kcache,
                         const void* vcache, const int32_t* page_table, int max_pages, const int32_t* seq_slot,
                         const int32_t* tok_pos, int B, int nh, int nkv, int splits, float* part_o, float* part_ml,
                         void* stream);
+/* The decode step's attention as the engine launches it: RoPE of the current token's q and k, its k / v appended to the
+ * cache at tok_pos, attention over the cache.  The raw q|k|v projection row of the token is either bf16 qkv [B][ld_qkv]
+ * (qkv_partial NULL) or the sum of fp32 split-K partials qkv_partial[s * split_stride + b * ld_partial + col],
+ * s < qkv_splits (qkv NULL), plus qkv_bias (bf16 [nh*128 + 2*nkv*128], partials only; NULL = none) before its bf16
+ * rounding.  cos_tab / sin_tab: bf16 [positions][64].  splits > 1: split_counter = device int32 [B * nkv], zero, selects
+ * the merge by the last-arriving CTA (left zero again); NULL selects the separate combine kernel. */
+int b200_op_attn_decode_fused(const void* qkv, int64_t ld_qkv, const float* qkv_partial, int qkv_splits, int64_t split_stride,
+                              int64_t ld_partial, const void* qkv_bias, const void* cos_tab, const void* sin_tab, void* out,
+                              int64_t ldo, void* kcache, void* vcache, const int32_t* page_table, int max_pages,
+                              const int32_t* seq_slot, const int32_t* tok_pos, int B, int nh, int nkv, int splits, float* part_o,
+                              float* part_ml, int32_t* split_counter, void* stream);
 int b200_op_rope_kv(const void* qkv, int64_t ld, void* q_out, int64_t ldq, void* kcache, void* vcache,
                     const int32_t* page_table, int max_pages, const int32_t* tok_seq, const int32_t* tok_pos,
                     const void* cos_tab, const void* sin_tab, int T, int nh, int nkv, void* stream);

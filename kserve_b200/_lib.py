@@ -75,8 +75,12 @@ def load() -> C.CDLL:
                                          C.c_int, C.c_int, vp]
     lib.b200_op_attn_prefill_tc.argtypes = [vp, i64, C.c_int, vp, i64, vp, vp, C.c_int, vp, C.c_int, vp, vp, C.c_int, C.c_int,
                                             C.c_int, C.c_int, vp]
+    lib.b200_op_attn_prefill_tc_off.argtypes = [vp, i64, C.c_int, vp, i64, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, C.c_int,
+                                                C.c_int, C.c_int, C.c_int, vp]
     lib.b200_op_attn_decode.argtypes = [vp, i64, vp, i64, vp, vp, vp, C.c_int, vp, vp, C.c_int, C.c_int,
                                         C.c_int, C.c_int, vp, vp, vp]
+    lib.b200_op_attn_decode_fused.argtypes = [vp, i64, vp, C.c_int, i64, i64, vp, vp, vp, vp, i64, vp, vp, vp, C.c_int, vp, vp,
+                                              C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
     lib.b200_op_rope_kv.argtypes = [vp, i64, vp, i64, vp, vp, vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int,
                                     C.c_int, vp]
     lib.b200_op_argmax.argtypes = [vp, i64, C.c_int, C.c_int, vp, vp, vp]

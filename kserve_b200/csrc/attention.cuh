@@ -22,13 +22,15 @@ constexpr int kTileBytes = kPageTokens * kHeadDim * 2;  // 16 KB
 // byte offset of 16-byte chunk `c` (0..15) of row `r` in a [rows][128] bf16 tile with XOR swizzle
 __device__ __forceinline__ uint32_t swz(int r, int c) { return (uint32_t)(r * 256 + ((c ^ (r & 7)) << 4)); }
 
-// stage one 64x128 bf16 tile (contiguous in global memory) into swizzled smem; 128 threads
-__device__ __forceinline__ void load_kv_tile(uint32_t sdst, const bf16* gsrc) {
+// stage one 64x128 bf16 tile (contiguous in global memory) into swizzled smem; 128 threads.  Rows >= valid_rows are
+// zero-filled instead of copied: a page's slots past the context hold whatever an earlier owner of the page left there
+// (possibly Inf / NaN), and a masked key's p = 0 times a NaN V row is still NaN inside the P.V MMA.
+__device__ __forceinline__ void load_kv_tile(uint32_t sdst, const bf16* gsrc, int valid_rows = kPageTokens) {
 #pragma unroll
   for (int it = 0; it < 8; ++it) {
     const int idx = threadIdx.x + it * kAttnThreads;
     const int r = idx >> 4, c = idx & 15;
-    cp_async_16(sdst + swz(r, c), gsrc + r * kHeadDim + c * 8, true);
+    cp_async_16(sdst + swz(r, c), gsrc + r * kHeadDim + c * 8, r < valid_rows);
   }
 }
 
@@ -232,7 +234,8 @@ __device__ __forceinline__ void attn_decode_arrive_and_merge(const AttnDecodePar
     for (int s = 0; s < p.splits; ++s) {
       const long long row = base + (long long)s * G + r;
       const float ms = __ldcg(p.part_ml + row * 2);
-      const float f = (ms == -INFINITY) ? 0.f : exp2f(ms - M);
+      if (ms == -INFINITY) continue;   // empty split: its part_o row was never written
+      const float f = exp2f(ms - M);
       L += __ldcg(p.part_ml + row * 2 + 1) * f;
       acc += __ldcg(p.part_o + row * kHeadDim + d) * f;
     }
@@ -279,8 +282,9 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const AttnDec
   for (int st = 0; st < kDecStages - 1; ++st) {
     if (t0 + st < t1) {
       const long long pg = pages[t0 + st];
-      load_kv_tile(sK + st * kTileBytes, p.kcache + pg * tile_stride + head_off);
-      load_kv_tile(sV + st * kTileBytes, p.vcache + pg * tile_stride + head_off);
+      const int rows = ctx - (t0 + st) * 64;   // > 0; rows past the context are zero-filled
+      load_kv_tile(sK + st * kTileBytes, p.kcache + pg * tile_stride + head_off, rows);
+      load_kv_tile(sV + st * kTileBytes, p.vcache + pg * tile_stride + head_off, rows);
     }
     cp_async_commit();
   }
@@ -389,8 +393,8 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const AttnDec
       if (jn < t1) {
         const int nb = (jn - t0) % kDecStages;
         const long long pg = pages[jn];
-        load_kv_tile(sK + nb * kTileBytes, p.kcache + pg * tile_stride + head_off);
-        load_kv_tile(sV + nb * kTileBytes, p.vcache + pg * tile_stride + head_off);
+        load_kv_tile(sK + nb * kTileBytes, p.kcache + pg * tile_stride + head_off, ctx - jn * 64);
+        load_kv_tile(sV + nb * kTileBytes, p.vcache + pg * tile_stride + head_off, ctx - jn * 64);
       }
       cp_async_commit();
     }
@@ -484,7 +488,8 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const AttnDec
 #pragma unroll
     for (int w = 0; w < 4; ++w) {
       const float mw = sm_m[w * 8 + r];
-      const float f = (mw == -INFINITY) ? 0.f : exp2f(mw - M);
+      if (mw == -INFINITY) continue;   // every key this warp saw was masked
+      const float f = exp2f(mw - M);
       L += sm_l[w * 8 + r] * f;
       acc += sm_o[(w * 8 + r) * kHeadDim + d] * f;
     }
@@ -518,7 +523,8 @@ attn_combine_kernel(const float* __restrict__ part_o, const float* __restrict__ 
   for (int s = 0; s < splits; ++s) {
     const long long row = base + (long long)s * G + r;
     const float ms = part_ml[row * 2];
-    const float f = (ms == -INFINITY) ? 0.f : exp2f(ms - M);
+    if (ms == -INFINITY) continue;   // empty split: its part_o row was never written
+    const float f = exp2f(ms - M);
     L += part_ml[row * 2 + 1] * f;
     acc += part_o[row * kHeadDim + d] * f;
   }

@@ -57,7 +57,12 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
   const int kvh = h / (p.nh / p.nkv);
   const int32_t* pages = p.page_table + (long long)p.seq_slot[b] * p.max_pages;
   const int off_tiles = p.kv_off ? (p.kv_off[b] >> 7) : 0;    // 128-token blocks that precede this chunk's first query row
-  const int ntiles = 2 * (off_tiles + qt + 1);                 // causal: 64-token KV tiles 0 .. 2 * (off_tiles + qt) + 1
+  const int ntiles_causal = 2 * (off_tiles + qt + 1);          // causal: 64-token KV tiles 0 .. 2 * (off_tiles + qt) + 1
+  // Keys [0, kv_end) exist.  The last query tile's second KV tile can lie wholly past kv_end: it is neither loaded nor
+  // multiplied (every p of it would be 0, so skipping it changes no bit).  The tile that straddles kv_end gets its V rows
+  // past the end zeroed before P.V (below): the page's tail is stale memory and 0 * NaN is NaN.
+  const int kv_end = off_tiles * 128 + len;
+  const int ntiles = min(ntiles_causal, (kv_end + kTcKv - 1) / kTcKv);
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_q); tma_prefetch_desc(&tmap_k); tma_prefetch_desc(&tmap_v);
@@ -128,7 +133,7 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
     if (t == 0) mbar_arrive(&k_empty[st]);
     // ---- online softmax; the softmax scale is folded into the exponent (max on the raw scores — the scale is
     // positive — then p = exp2(fma(s, scale, -m)): one FFMA per element)
-    if (j >= ntiles - 2) {
+    if (j >= ntiles_causal - 2) {
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
         const int key = j * kTcKv + 8 * (i >> 2) + col_t + (i & 1);
@@ -162,6 +167,17 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
     for (int i = 0; i < 64; ++i) o[i] *= corr[(i >> 1) & 1];
     // ---- O += P V: 16 tokens per MMA; the S fragment of tokens [16k, 16k + 16) is the A fragment {pa[4k] .. pa[4k + 3]}
     mbar_wait(&v_full[st], ph);
+    if (kv_end < (j + 1) * kTcKv) {   // the tile straddling kv_end (uniform per CTA): zero its V rows past the end
+      // a 128B-swizzled row keeps its 128 bytes, so row r of each [64 x 64] box is bytes [128 r, 128 r + 128)
+      uint8_t* vd = sV + st * kTcTile;
+      const int r0 = kv_end - j * kTcKv;
+      for (int i = threadIdx.x - 128; i < (kTcKv - r0) * 16; i += 256) {   // 16 B chunks: 8 per row in each of the 2 boxes
+        const int row = r0 + (i >> 4), box = (i >> 3) & 1, c = i & 7;
+        *reinterpret_cast<uint4*>(vd + box * (kTcTile / 2) + row * 128 + c * 16) = make_uint4(0u, 0u, 0u, 0u);
+      }
+      fence_proxy_async_shared();                      // generic-proxy stores -> visible to wgmma
+      asm volatile("bar.sync 1, 256;" ::: "memory");   // both consumer warpgroups
+    }
     {
       const uint32_t vb = smem_u32(sV + st * kTcTile);
       wgmma_fence();

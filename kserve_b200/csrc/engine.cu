@@ -2349,16 +2349,25 @@ int b200_op_attn_prefill(const void* q, int64_t ldq, void* out, int64_t ldo, con
   return launch_attn_prefill(p, B, max_len, (cudaStream_t)stream);
 }
 
-int b200_op_attn_prefill_tc(const void* q, int64_t ldq, int q_rows, void* out, int64_t ldo, const void* kcache,
-                            const void* vcache, int num_pages, const int32_t* page_table, int max_pages,
-                            const int32_t* cu_seqlens, const int32_t* seq_slot, int B, int max_len, int nh, int nkv,
-                            void* stream) {
+int b200_op_attn_prefill_tc_off(const void* q, int64_t ldq, int q_rows, void* out, int64_t ldo, const void* kcache,
+                                const void* vcache, int num_pages, const int32_t* page_table, int max_pages,
+                                const int32_t* cu_seqlens, const int32_t* seq_slot, const int32_t* kv_off, int B, int max_len,
+                                int nh, int nkv, void* stream) {
   g_op_tmaps.maps.clear();
   AttnTcParams p{};
   p.out = (bf16*)out; p.ldo = ldo; p.page_table = page_table; p.max_pages = max_pages; p.cu_seqlens = cu_seqlens;
   p.seq_slot = seq_slot; p.nh = nh; p.nkv = nkv; p.scale_log2 = (1.0f / sqrtf((float)kHeadDim)) * 1.4426950408889634f;
+  p.kv_off = kv_off;
   return launch_attn_prefill_tc(g_op_tmaps, (const bf16*)q, q_rows, ldq, (const bf16*)kcache, (const bf16*)vcache, num_pages, p, B,
                                 max_len, (cudaStream_t)stream);
+}
+
+int b200_op_attn_prefill_tc(const void* q, int64_t ldq, int q_rows, void* out, int64_t ldo, const void* kcache,
+                            const void* vcache, int num_pages, const int32_t* page_table, int max_pages,
+                            const int32_t* cu_seqlens, const int32_t* seq_slot, int B, int max_len, int nh, int nkv,
+                            void* stream) {
+  return b200_op_attn_prefill_tc_off(q, ldq, q_rows, out, ldo, kcache, vcache, num_pages, page_table, max_pages, cu_seqlens,
+                                     seq_slot, nullptr, B, max_len, nh, nkv, stream);
 }
 
 int b200_op_attn_decode(const void* q, int64_t ldq, void* out, int64_t ldo, const void* kcache, const void* vcache,
@@ -2369,6 +2378,26 @@ int b200_op_attn_decode(const void* q, int64_t ldq, void* out, int64_t ldo, cons
   p.page_table = page_table; p.max_pages = max_pages; p.seq_slot = seq_slot; p.tok_pos = tok_pos; p.nh = nh; p.nkv = nkv;
   p.G = nh / nkv; p.splits = splits; p.part_o = part_o; p.part_ml = part_ml;
   p.scale_log2 = (1.0f / sqrtf((float)kHeadDim)) * 1.4426950408889634f;
+  return launch_attn_decode(p, B, (cudaStream_t)stream);
+}
+
+int b200_op_attn_decode_fused(const void* qkv, int64_t ld_qkv, const float* qkv_partial, int qkv_splits, int64_t split_stride,
+                              int64_t ld_partial, const void* qkv_bias, const void* cos_tab, const void* sin_tab, void* out,
+                              int64_t ldo, void* kcache, void* vcache, const int32_t* page_table, int max_pages,
+                              const int32_t* seq_slot, const int32_t* tok_pos, int B, int nh, int nkv, int splits, float* part_o,
+                              float* part_ml, int32_t* split_counter, void* stream) {
+  B200_REQUIRE((qkv == nullptr) != (qkv_partial == nullptr), "exactly one of qkv / qkv_partial must be given");
+  B200_REQUIRE(qkv_bias == nullptr || qkv_partial != nullptr, "qkv_bias applies to split-K partials only");
+  AttnDecodeParams p{};
+  p.out = (bf16*)out; p.ldo = ldo; p.kcache = (const bf16*)kcache; p.vcache = (const bf16*)vcache;
+  p.page_table = page_table; p.max_pages = max_pages; p.seq_slot = seq_slot; p.tok_pos = tok_pos; p.nh = nh; p.nkv = nkv;
+  p.G = nh / nkv; p.splits = splits; p.part_o = part_o; p.part_ml = part_ml;
+  p.scale_log2 = (1.0f / sqrtf((float)kHeadDim)) * 1.4426950408889634f;
+  p.fuse_rope = 1; p.qkv = (const bf16*)qkv; p.ld_qkv = ld_qkv;
+  p.qkv_partial = qkv_partial; p.qkv_splits = qkv_splits; p.qkv_split_stride = split_stride; p.ld_qkv_partial = ld_partial;
+  p.qkv_bias = (const bf16*)qkv_bias; p.cos_tab = (const bf16*)cos_tab; p.sin_tab = (const bf16*)sin_tab;
+  p.kcache_w = (bf16*)kcache; p.vcache_w = (bf16*)vcache;
+  p.split_counter = split_counter;
   return launch_attn_decode(p, B, (cudaStream_t)stream);
 }
 

@@ -303,3 +303,53 @@ def test_kv_host_offload_tier_roundtrip(engines):
         eng.kv_swap_in(b)
     eng.run_staged(False, T - 1 - 9)
     assert torch.equal(eng.fetch_staged(), ref)
+
+
+def test_long_context_3968_prompt_tokens():
+    """A 3968-token prompt (31 query tiles of 128) plus 64 generated tokens on tiny_g2_rope3, whose max_position of 4096
+    bounds both: every step's logits against the oracle's forward (on the CPU) over the engine's own ids, at the stated
+    tolerance; then the same greedy ids through the continuous batcher with 1024-token prefill chunks and the prefix
+    cache, alongside a second prompt that shares the first 2048 tokens (chunks start at kv_off 1024 ... 3072)."""
+    from oracle import weights as W
+    from oracle.hf_oracle import OracleGenerativeModel, build_model
+    S, T, pad = 3968, 64, 1030
+    g = torch.Generator().manual_seed(3968)
+    ids = torch.randint(3, 1000, (1, S), generator=g)
+    other = ids.clone()
+    other[0, 2048:] = torch.randint(3, 1000, (S - 2048,), generator=g)
+    eng = make_engine("tiny_g2_rope3", 0, max_batch=2, max_seq_len=S + T)
+    try:
+        r = eng.generate(ids, None, max_new_tokens=T, pad_token_id=pad, want_logits=True)
+        assert r.num_generated == T
+        ref_other = eng.generate(other, None, max_new_tokens=T, pad_token_id=pad).output_ids[0, S:].tolist()
+        cfg = W.CONFIGS["tiny_g2_rope3"]
+        orc = OracleGenerativeModel(build_model(cfg, W.synth_state_dict(cfg, 0)), pad_token_id=pad)
+        ref = orc.forward_logits(r.output_ids[:, :-1])[:, S - 1:]          # [1, T, V]: step t sees prompt + t engine ids
+        got = r.logits.float().permute(1, 0, 2)
+        tol = logits_tol(ref)
+        err = float((got - ref).abs().max())
+        _record("long_context_3968:teacher_forced", max_err=err, tol=tol)
+        assert err <= tol, f"max logits error {err:.4f} > tol {tol:.4f}"
+
+        eng.cb_begin(pad, [])
+        eng.cb_config(1024, True)
+        try:
+            a = eng.cb_admit([ids[0].tolist()], [T])[0]
+            for _ in range(T + 8):
+                if eng.cb_poll()[1][a]:
+                    break
+                eng.cb_step(1)
+            assert eng.cb_read(a, 0, T) == r.output_ids[0, S:].tolist()
+            eng.cb_release(a)
+            b = eng.cb_admit([other[0].tolist()], [T])[0]
+            assert eng.cb_stats()["prefix_hit_tokens"] == 2048
+            for _ in range(T + 8):
+                if eng.cb_poll()[1][b]:
+                    break
+                eng.cb_step(1)
+            assert eng.cb_read(b, 0, T) == ref_other
+            eng.cb_release(b)
+        finally:
+            eng.cb_end()
+    finally:
+        eng.close()

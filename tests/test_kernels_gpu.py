@@ -248,7 +248,7 @@ def test_attn_prefill(lib, nh, nkv, lens):
         t0 += l
 
 
-@pytest.mark.parametrize("nh,nkv", [(4, 2), (8, 2), (32, 8)])
+@pytest.mark.parametrize("nh,nkv", [(4, 2), (8, 2), (32, 8), (8, 8), (12, 2), (28, 4), (64, 8)])
 @pytest.mark.parametrize("lens", [[5], [64, 1, 130], [200, 63, 65, 128, 129], [700, 257]])
 def test_attn_prefill_tcgen05(lib, nh, nkv, lens):
     """The wgmma prefill attention (engine default) against the fp32 statement of causal GQA attention."""
@@ -270,8 +270,8 @@ def test_attn_prefill_tcgen05(lib, nh, nkv, lens):
         t0 += l
 
 
-@pytest.mark.parametrize("nh,nkv", [(4, 2), (8, 2), (32, 8)])
-@pytest.mark.parametrize("splits", [1, 2, 5])
+@pytest.mark.parametrize("nh,nkv", [(4, 2), (8, 2), (32, 8), (8, 8), (40, 8), (28, 4), (64, 8)])
+@pytest.mark.parametrize("splits", [1, 2, 5, 8])
 def test_attn_decode(lib, nh, nkv, splits):
     lens = [1, 64, 65, 200, 1000, 17]
     B = len(lens)
