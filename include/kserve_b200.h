@@ -48,6 +48,10 @@ typedef struct b200_model_config {
   int32_t weight_format;       /* 0 = bf16; 1 = FP8: the q/k/v/o and gate/up/down projections are float8_e4m3fn codes with
                                 * one scale per weight row (b200_engine_set_weight_fp8); dense models on one GPU only
                                 * (tp_size 1) */
+  int32_t kv_cache_dtype;      /* 0 = bf16 KV pages, [page][kv_head][64][128] x 2 bytes; 1 = float8_e4m3fn codes, 1 byte each
+                                * (16 KB -> 8 KB per (page, kv head) tile): k after RoPE and v are stored as
+                                * e4m3(clamp(bf16 value, -448, 448)) rounded to nearest even (per-tensor scale 1), attention
+                                * reads them back exactly as bf16.  Not with tp_size > 1 or B200_ATTN_MMA=1 */
 } b200_model_config_t;
 
 /* Creates the engine on cfg->device. nccl_unique_id: 128 bytes shared by all ranks (from
@@ -213,6 +217,11 @@ int b200_op_attn_prefill_tc_off(const void* q, int64_t ldq, int q_rows, void* ou
                                 const void* vcache, int num_pages, const int32_t* page_table, int max_pages,
                                 const int32_t* cu_seqlens, const int32_t* seq_slot, const int32_t* kv_off, int B, int max_len,
                                 int nh, int nkv, void* stream);
+/* b200_op_attn_prefill_tc_off on caches of float8_e4m3fn codes (kv_cache_dtype 1): attention reads bf16(code) */
+int b200_op_attn_prefill_tc_kv8(const void* q, int64_t ldq, int q_rows, void* out, int64_t ldo, const void* kcache,
+                                const void* vcache, int num_pages, const int32_t* page_table, int max_pages,
+                                const int32_t* cu_seqlens, const int32_t* seq_slot, const int32_t* kv_off, int B, int max_len,
+                                int nh, int nkv, void* stream);
 /* decode attention on already-roped queries (q [B][ldq]); splits > 1 merges with a separate combine kernel */
 int b200_op_attn_decode(const void* q, int64_t ldq, void* out, int64_t ldo, const void* kcache,
                         const void* vcache, const int32_t* page_table, int max_pages, const int32_t* seq_slot,
@@ -229,6 +238,14 @@ int b200_op_attn_decode_fused(const void* qkv, int64_t ld_qkv, const float* qkv_
                               int64_t ldo, void* kcache, void* vcache, const int32_t* page_table, int max_pages,
                               const int32_t* seq_slot, const int32_t* tok_pos, int B, int nh, int nkv, int splits, float* part_o,
                               float* part_ml, int32_t* split_counter, void* stream);
+/* b200_op_attn_decode_fused on caches of float8_e4m3fn codes (kv_cache_dtype 1): appends e4m3(k), e4m3(v) and attends
+ * over bf16(code), the current token included */
+int b200_op_attn_decode_fused_kv8(const void* qkv, int64_t ld_qkv, const float* qkv_partial, int qkv_splits,
+                                  int64_t split_stride, int64_t ld_partial, const void* qkv_bias, const void* cos_tab,
+                                  const void* sin_tab, void* out, int64_t ldo, void* kcache, void* vcache,
+                                  const int32_t* page_table, int max_pages, const int32_t* seq_slot, const int32_t* tok_pos,
+                                  int B, int nh, int nkv, int splits, float* part_o, float* part_ml, int32_t* split_counter,
+                                  void* stream);
 int b200_op_rope_kv(const void* qkv, int64_t ld, void* q_out, int64_t ldq, void* kcache, void* vcache,
                     const int32_t* page_table, int max_pages, const int32_t* tok_seq, const int32_t* tok_pos,
                     const void* cos_tab, const void* sin_tab, int T, int nh, int nkv, void* stream);

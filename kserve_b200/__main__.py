@@ -27,6 +27,9 @@ def main(argv=None):
                         help="with --continuous_batching: prompts are prefilled in chunks of this many tokens between decode steps (0 = whole prompts at admit)")
     parser.add_argument("--enable_prefix_caching", action="store_true",
                         help="with --continuous_batching: share the KV pages of common 128-token prompt prefixes between requests")
+    parser.add_argument("--kv_cache_dtype", default="auto", choices=["auto", "bfloat16", "fp8", "fp8_e4m3", "fp8_e5m2"],
+                        help="KV cache element type: auto / bfloat16 = bf16 pages; fp8 / fp8_e4m3 = float8_e4m3fn codes (per-tensor "
+                             "scale 1), half the bytes per cached token (fp8_e5m2 is refused)")
     parser.add_argument("--tensor_parallel_size", type=int, default=int(os.environ.get("WORLD_SIZE", "1")))
     # the agent's flags (cmd/agent/main.go:66-68 --enable-batcher / --max-batchsize / --max-latency), same defaults
     parser.add_argument("--enable_batcher", "--enable-batcher", dest="enable_batcher", action="store_true",
@@ -36,6 +39,8 @@ def main(argv=None):
     args, _ = parser.parse_known_args(argv)
     if args.dtype not in ("auto", "bfloat16"):
         parser.error(f"--dtype {args.dtype}: the H100 runtime computes in bfloat16 only (use --dtype auto or bfloat16)")
+    if args.kv_cache_dtype == "fp8_e5m2":
+        parser.error("--kv_cache_dtype fp8_e5m2 is not supported: the FP8 KV cache is float8_e4m3fn (use fp8 or fp8_e4m3)")
     if args.enable_batcher and (args.max_batchsize <= 0 or args.max_latency <= 0):
         parser.error("Invalid max batch size / max latency")        # cmd/agent/main.go:256-273
     from .generative_model import B200GenerativeModel
@@ -52,7 +57,8 @@ def main(argv=None):
         args.max_batch = max(args.max_batch, min(args.max_batchsize, 64))     # a formed batch must fit one engine call
     model = B200GenerativeModel(args.model_name, path, max_model_len=args.max_model_len, max_batch=args.max_batch,
                                 device=int(os.environ.get("LOCAL_RANK", "0")), tensor_parallel_size=args.tensor_parallel_size,
-                                tp_rank=rank, nccl_id=nccl_id, continuous_batching=args.continuous_batching)
+                                tp_rank=rank, nccl_id=nccl_id, continuous_batching=args.continuous_batching,
+                                kv_cache_dtype=args.kv_cache_dtype)
     model.prefill_chunk_tokens, model.prefix_cache = max(0, args.prefill_chunk_tokens), args.enable_prefix_caching
     model.load()
     if rank != 0:

@@ -14,7 +14,8 @@ class ModelConfig(C.Structure):
         "vocab_size", "hidden_size", "intermediate_size", "num_layers", "num_heads", "num_kv_heads",
         "head_dim", "max_position")] + [("rms_eps", C.c_float), ("rope_theta", C.c_float)] + [
         (n, C.c_int32) for n in ("max_batch", "max_seq_len", "max_prefill_tokens", "num_kv_pages",
-                                 "tp_rank", "tp_size", "device", "num_experts", "num_experts_per_tok", "weight_format")]
+                                 "tp_rank", "tp_size", "device", "num_experts", "num_experts_per_tok", "weight_format",
+                                 "kv_cache_dtype")]
 
 
 class GenParams(C.Structure):

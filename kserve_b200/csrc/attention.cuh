@@ -9,8 +9,13 @@
 // 16 KB block that is staged with 128-bit cp.async into XOR-swizzled shared memory and consumed with
 // ldmatrix + mma.sync.m16n8k16 (fp32 softmax / accumulation).  This round's kernels use the legacy
 // warp-level MMA path; they are HBM-bound in decode (the KV read) and 2% of prefill FLOPs.
+//
+// FP8 KV cache (attn_decode_kernel<true>): pages hold e4m3 codes, [page][kv_head][64][128] bytes, so a tile is 8 KB.  The
+// codes go through a cp.async ring of their own and the CTA expands each tile (exactly: every e4m3 value is a bf16
+// value) into the same swizzled bf16 tile as above, so the MMA loop and the merges are the bf16 kernel's.
 #pragma once
 #include "common.cuh"
+#include "gemm_wgmma.cuh"
 #include "ops.cuh"
 
 namespace b200 {
@@ -18,6 +23,8 @@ namespace b200 {
 constexpr int kAttnThreads = 128;
 constexpr int kDecStages = 3;   // cp.async ring of the decode kernel: two KV tiles (64 KB) in flight per CTA
 constexpr int kTileBytes = kPageTokens * kHeadDim * 2;  // 16 KB
+constexpr int kDecStages8 = 4;  // FP8 KV: code ring of 4 (K, V) stages = 64 KB, + one bf16 K and V tile = the bf16 ring's 96 KB
+constexpr int kTile8Bytes = kPageTokens * kHeadDim;     // 8 KB of e4m3 codes
 
 // byte offset of 16-byte chunk `c` (0..15) of row `r` in a [rows][128] bf16 tile with XOR swizzle
 __device__ __forceinline__ uint32_t swz(int r, int c) { return (uint32_t)(r * 256 + ((c ^ (r & 7)) << 4)); }
@@ -31,6 +38,30 @@ __device__ __forceinline__ void load_kv_tile(uint32_t sdst, const bf16* gsrc, in
     const int idx = threadIdx.x + it * kAttnThreads;
     const int r = idx >> 4, c = idx & 15;
     cp_async_16(sdst + swz(r, c), gsrc + r * kHeadDim + c * 8, r < valid_rows);
+  }
+}
+
+// stage one 64x128 tile of e4m3 codes into an unswizzled [64][128 B] buffer; rows >= valid_rows zero-filled (code 0 = +0)
+__device__ __forceinline__ void load_kv_tile8(uint32_t sdst, const uint8_t* gsrc, int valid_rows) {
+#pragma unroll
+  for (int it = 0; it < 4; ++it) {
+    const int idx = threadIdx.x + it * kAttnThreads;
+    const int r = idx >> 3, c = idx & 7;
+    cp_async_16(sdst + r * 128 + c * 16, gsrc + r * 128 + c * 16, r < valid_rows);
+  }
+}
+
+// expand a staged code tile into the swizzled bf16 tile load_kv_tile would have produced from bf16(codes); 128 threads
+__device__ __forceinline__ void expand_kv_tile8(uint8_t* dst, const uint8_t* codes) {
+  const Fp8Scale one = fp8_scale(__float2bfloat16(1.0f));
+#pragma unroll
+  for (int it = 0; it < 4; ++it) {
+    const int idx = threadIdx.x + it * kAttnThreads;
+    const int r = idx >> 3, c = idx & 7;
+    uint4 o0, o1;
+    fp8x16_dequant(*reinterpret_cast<const uint4*>(codes + r * 128 + c * 16), one, o0, o1);
+    *reinterpret_cast<uint4*>(dst + swz(r, 2 * c)) = o0;
+    *reinterpret_cast<uint4*>(dst + swz(r, 2 * c + 1)) = o1;
   }
 }
 
@@ -190,7 +221,7 @@ __global__ void __launch_bounds__(kAttnThreads) attn_prefill_kernel(const AttnPr
 struct AttnDecodeParams {
   const bf16* q; long long ldq;        // [B][ldq] roped queries of the current token
   bf16* out; long long ldo;            // [B][ldo]
-  const bf16* kcache; const bf16* vcache;
+  const bf16* kcache; const bf16* vcache;   // e4m3 codes (one byte per element) in attn_decode_kernel<true>
   const int32_t* page_table; int max_pages;
   const int32_t* seq_slot;             // [B]
   const int32_t* tok_pos;              // [B] position of the current token; context = pos + 1
@@ -208,7 +239,7 @@ struct AttnDecodeParams {
   const bf16* qkv_bias;   // [ld_qkv] projection bias added to the summed partials before their bf16 rounding (nullptr = none;
                           // a bf16 `qkv` row already carries it from the GEMM epilogue)
   const bf16* cos_tab; const bf16* sin_tab;
-  bf16* kcache_w; bf16* vcache_w;
+  bf16* kcache_w; bf16* vcache_w;       // (e4m3 codes in attn_decode_kernel<true>, which appends e4m3(k), e4m3(v))
   // splits > 1: per-(sequence, kv head) arrival counters (zero between launches).  When set, the LAST split CTA to
   // arrive merges the partials itself (in split order: deterministic) and no attn_combine_kernel follows — one kernel
   // boundary less on the tensor-parallel decode path, where few (sequence, kv head) pairs per GPU force the split.
@@ -243,7 +274,9 @@ __device__ __forceinline__ void attn_decode_arrive_and_merge(const AttnDecodePar
   }
 }
 
+template <bool KV8>
 __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const AttnDecodeParams p) {
+  constexpr int STAGES = KV8 ? kDecStages8 : kDecStages;
   TraceScope _ts(TK_ATTN_DECODE);
   pdl_launch_dependents();
   pdl_wait();
@@ -266,8 +299,9 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const AttnDec
     return;
   }
   const uint32_t sQ = smem_u32(smem);       // 16 rows x 256 B = 4 KB
-  const uint32_t sK = sQ + 4096;                      // kDecStages x 16 KB
-  const uint32_t sV = sK + kDecStages * kTileBytes;   // kDecStages x 16 KB
+  const uint32_t sK = sQ + 4096;                      // bf16: kDecStages x 16 KB; KV8: the one expanded 16 KB tile
+  const uint32_t sV = sK + (KV8 ? 1 : kDecStages) * kTileBytes;
+  const uint32_t s8 = sQ + 4096 + 2 * kTileBytes;     // KV8: code ring, stage st = K codes at st * 16 KB, V codes 8 KB after
   const int32_t* pages = p.page_table + (long long)p.seq_slot[b] * p.max_pages;
   const long long tile_stride = (long long)p.nkv * kPageTokens * kHeadDim;
   const long long head_off = (long long)kvh * kPageTokens * kHeadDim;
@@ -277,15 +311,23 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const AttnDec
   float* s_raw = reinterpret_cast<float*>(smem + 4096 + 2 * kDecStages * kTileBytes);   // [(G+2)][128] fp32
   bf16* s_newk = reinterpret_cast<bf16*>(s_raw + 10 * kHeadDim);           // [128]
   bf16* s_newv = s_newk + kHeadDim;                                          // [128]
-  // fill the ring: kDecStages-1 tiles in flight before any compute (one commit group per ring slot, empty or not)
-#pragma unroll
-  for (int st = 0; st < kDecStages - 1; ++st) {
-    if (t0 + st < t1) {
-      const long long pg = pages[t0 + st];
-      const int rows = ctx - (t0 + st) * 64;   // > 0; rows past the context are zero-filled
+  const uint8_t* kc8 = reinterpret_cast<const uint8_t*>(p.kcache);
+  const uint8_t* vc8 = reinterpret_cast<const uint8_t*>(p.vcache);
+  // stage tile jt into ring slot st; rows past the context are zero-filled
+  auto load_stage = [&](int st, int jt_, int rows) {
+    const long long pg = pages[jt_];
+    if constexpr (KV8) {
+      load_kv_tile8(s8 + st * 2 * kTile8Bytes, kc8 + pg * tile_stride + head_off, rows);
+      load_kv_tile8(s8 + st * 2 * kTile8Bytes + kTile8Bytes, vc8 + pg * tile_stride + head_off, rows);
+    } else {
       load_kv_tile(sK + st * kTileBytes, p.kcache + pg * tile_stride + head_off, rows);
       load_kv_tile(sV + st * kTileBytes, p.vcache + pg * tile_stride + head_off, rows);
     }
+  };
+  // fill the ring: STAGES-1 tiles in flight before any compute (one commit group per ring slot, empty or not)
+#pragma unroll
+  for (int st = 0; st < STAGES - 1; ++st) {
+    if (t0 + st < t1) load_stage(st, t0 + st, ctx - (t0 + st) * 64);   // rows > 0
     cp_async_commit();
   }
   if (p.fuse_rope) {
@@ -338,6 +380,10 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const AttnDec
           const float x1 = s_raw[hl * kHeadDim + c + i], x2 = s_raw[hl * kHeadDim + c + 64 + i];
           o1[i] = bf16_round(x1 * cs[i]) + bf16_round(-x2 * sn[i]);
           o2[i] = bf16_round(x2 * cs[i]) + bf16_round(x1 * sn[i]);
+          if (KV8 && hl == G) {   // the new k as the cache will give it back
+            o1[i] = e4m3_roundtrip(bf16_round(o1[i]));
+            o2[i] = e4m3_roundtrip(bf16_round(o2[i]));
+          }
         }
         if (hl < G) {
           *reinterpret_cast<uint4*>(smem + swz(hl, c >> 3)) = pack8(o1);
@@ -350,7 +396,7 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const AttnDec
         const int c = (it - (G + 1) * 8) * 8;
         float f[8];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) f[i] = s_raw[(G + 1) * kHeadDim + c + i];
+        for (int i = 0; i < 8; ++i) f[i] = KV8 ? e4m3_roundtrip(s_raw[(G + 1) * kHeadDim + c + i]) : s_raw[(G + 1) * kHeadDim + c + i];
         *reinterpret_cast<uint4*>(s_newv + c) = pack8(f);
       }
     }
@@ -361,8 +407,13 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const AttnDec
     if (jt >= t0 && jt < t1 && threadIdx.x < 32) {   // the split that owns the current token appends it to the cache
       const int c = (threadIdx.x & 15) * 8, slot = pos & 63;
       const long long off = (long long)pages[jt] * tile_stride + head_off + slot * kHeadDim + c;
-      if (threadIdx.x < 16) *reinterpret_cast<uint4*>(p.kcache_w + off) = *reinterpret_cast<const uint4*>(s_newk + c);
-      else *reinterpret_cast<uint4*>(p.vcache_w + off) = *reinterpret_cast<const uint4*>(s_newv + c);
+      if constexpr (KV8) {   // s_newk / s_newv hold e4m3 values: converting them back gives their codes exactly
+        uint8_t* dst = reinterpret_cast<uint8_t*>(threadIdx.x < 16 ? p.kcache_w : p.vcache_w) + off;
+        *reinterpret_cast<uint2*>(dst) = bf16x8_to_e4m3(*reinterpret_cast<const uint4*>((threadIdx.x < 16 ? s_newk : s_newv) + c));
+      } else {
+        if (threadIdx.x < 16) *reinterpret_cast<uint4*>(p.kcache_w + off) = *reinterpret_cast<const uint4*>(s_newk + c);
+        else *reinterpret_cast<uint4*>(p.vcache_w + off) = *reinterpret_cast<const uint4*>(s_newv + c);
+      }
     }
   } else {
     // Q: G rows valid, the rest zero
@@ -385,17 +436,12 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const AttnDec
   float m0 = -INFINITY, l0 = 0.f;  // only row g (< 8) matters: rows >= G are padding
 
   for (int j = t0; j < t1; ++j) {
-    const int buf = (j - t0) % kDecStages;
-    cp_async_wait<kDecStages - 2>();   // tile j has landed
-    __syncthreads();                   // ... for every thread, and everyone is done with tile j-1's slot
+    const int buf = (j - t0) % STAGES;
+    cp_async_wait<STAGES - 2>();   // tile j has landed
+    __syncthreads();               // ... for every thread, and everyone is done with tile j-1's slot
     {
-      const int jn = j + kDecStages - 1;   // refill the slot tile j-1 used
-      if (jn < t1) {
-        const int nb = (jn - t0) % kDecStages;
-        const long long pg = pages[jn];
-        load_kv_tile(sK + nb * kTileBytes, p.kcache + pg * tile_stride + head_off, ctx - jn * 64);
-        load_kv_tile(sV + nb * kTileBytes, p.vcache + pg * tile_stride + head_off, ctx - jn * 64);
-      }
+      const int jn = j + STAGES - 1;   // refill the slot tile j-1 used
+      if (jn < t1) load_stage((jn - t0) % STAGES, jn, ctx - jn * 64);
       cp_async_commit();
     }
     if (j == t0) {
@@ -403,16 +449,24 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const AttnDec
       for (int ks = 0; ks < 8; ++ks)
         ldmatrix_x4(qf[ks], sQ + swz((lane & 7) + 8 * ((lane >> 3) & 1), 2 * ks + (lane >> 4)));
     }
-    const uint32_t sKb = sK + buf * kTileBytes, sVb = sV + buf * kTileBytes;
+    const int tb = KV8 ? 0 : buf;   // bf16 tile the MMAs read
+    const uint32_t sKb = sK + tb * kTileBytes, sVb = sV + tb * kTileBytes;
+    if constexpr (KV8) {
+      const uint8_t* codes = smem + 4096 + 2 * kTileBytes + buf * 2 * kTile8Bytes;
+      expand_kv_tile8(smem + 4096, codes);
+      expand_kv_tile8(smem + 4096 + kTileBytes, codes + kTile8Bytes);
+      if (p.fuse_rope && j == jt) __syncthreads();   // the patch below overwrites an expanded row
+    }
     if (p.fuse_rope && j == jt) {   // the row of the current token is not in the cache copy that was just staged
       if (threadIdx.x < 32) {
         const int c = threadIdx.x & 15, slot = pos & 63;
-        uint8_t* base = smem + 4096 + (threadIdx.x < 16 ? 0 : kDecStages * kTileBytes) + buf * kTileBytes;
+        uint8_t* base = smem + 4096 + (threadIdx.x < 16 ? 0 : (KV8 ? 1 : kDecStages) * kTileBytes) + tb * kTileBytes;
         *reinterpret_cast<uint4*>(base + swz(slot, c)) =
             *reinterpret_cast<const uint4*>((threadIdx.x < 16 ? s_newk : s_newv) + c * 8);
       }
-      __syncthreads();
+      if (!KV8) __syncthreads();
     }
+    if (KV8) __syncthreads();       // the expanded (and patched) tile is complete
     float s[2][4];
     s[0][0] = s[0][1] = s[0][2] = s[0][3] = 0.f;
     s[1][0] = s[1][1] = s[1][2] = s[1][3] = 0.f;

@@ -9,8 +9,14 @@
 //                    fragment layout is the A fragment layout, so P never goes through shared memory — and V as an
 //                    MN-major shared-memory operand), finally O / l stored as bf16.
 // The two consumer warpgroups run independently, so one's softmax overlaps the other's tensor-core work.
+//
+// FP8 KV cache (attn_prefill_tc_kernel<true>): the cache holds e4m3 codes.  TMA brings each K / V tile as codes (an 8 KB
+// [64 tokens][128 B] box) into a 2-stage code ring, and the 128 threads of warpgroup 0 expand it (exactly) into the same
+// 128B-swizzled bf16 boxes the consumers read, writing the V rows past the end of the keys as zeros.  The consumers'
+// code is the bf16 kernel's; the conversion stays off their critical path.
 #pragma once
 #include "common.cuh"
+#include "gemm_wgmma.cuh"
 #include "ops.cuh"
 
 namespace b200 {
@@ -21,6 +27,25 @@ constexpr int kTcTile = 128 * 64 * 2;        // one [128 x 64] bf16 swizzled til
 // Q 2 tiles + K ring 2 stages + V ring 2 stages = 96 KB, + alignment slack and barriers; one CTA per SM
 constexpr int kTcSmem = 2 * kTcTile /*Q*/ + 2 * kTcTile /*K ring*/ + 2 * kTcTile /*V ring*/ + 1024 + 256;
 constexpr int kTcThreads = 384;
+constexpr int kTcTile8 = 64 * 128;           // one K or V tile of e4m3 codes = 8 KB
+constexpr int kTcSmem8 = kTcSmem + 2 * 2 * kTcTile8;   // + code ring[2] x {K, V}
+
+// warpgroup 0 (128 threads): codes [64 tokens][128 B] -> the two 128B-swizzled [64 x 64] bf16 boxes of a K / V stage;
+// rows >= valid_rows become zeros
+__device__ __forceinline__ void expand_tc_tile8(uint8_t* dst, const uint8_t* codes, int valid_rows) {
+  const Fp8Scale one = fp8_scale(__float2bfloat16(1.0f));
+#pragma unroll
+  for (int it = 0; it < 4; ++it) {
+    const int idx = threadIdx.x + it * 128;
+    const int r = idx >> 3, c = idx & 7;            // codes of dims [16 c, 16 c + 16) of token r
+    uint4 o0 = make_uint4(0u, 0u, 0u, 0u), o1 = o0;
+    if (r < valid_rows) fp8x16_dequant(*reinterpret_cast<const uint4*>(codes + r * 128 + c * 16), one, o0, o1);
+    uint8_t* row = dst + (c >> 2) * (kTcTile / 2) + r * 128;   // box (c >> 2), its 16-byte chunks 2 (c & 3) and + 1
+    const int cc = 2 * (c & 3);
+    *reinterpret_cast<uint4*>(row + ((cc ^ (r & 7)) << 4)) = o0;
+    *reinterpret_cast<uint4*>(row + (((cc + 1) ^ (r & 7)) << 4)) = o1;
+  }
+}
 
 struct AttnTcParams {
   bf16* out; long long ldo;
@@ -34,6 +59,8 @@ struct AttnTcParams {
   const int32_t* kv_off;
 };
 
+// KV8: tmap_k / tmap_v are maps over the e4m3 caches, box [64][128 B] (else bf16, box [64][64], 128B swizzle)
+template <bool KV8>
 __global__ void __launch_bounds__(kTcThreads, 1)
 attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                        const __grid_constant__ CUtensorMap tmap_v, const AttnTcParams p) {
@@ -43,8 +70,10 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
   uint8_t* sQ = smem;                       // 2 tiles (dims 0-63 | 64-127), 128 rows each
   uint8_t* sK = sQ + 2 * kTcTile;           // ring[2] x {dims 0-63 | 64-127} x 64 tokens
   uint8_t* sV = sK + 2 * kTcTile;           // ring[2], same shape
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * kTcTile);
+  uint8_t* s8 = sV + 2 * kTcTile;           // KV8: code ring[2] x {K, V}
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s8 + (KV8 ? 2 * 2 * kTcTile8 : 0));
   uint64_t *q_full = bars, *k_full = bars + 1, *k_empty = bars + 3, *v_full = bars + 5, *v_empty = bars + 7;
+  uint64_t* c_full = bars + 9;              // KV8: codes of stage st have landed
 
   const int b = blockIdx.z, h = blockIdx.y, qt = blockIdx.x;
   const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -68,13 +97,48 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
     tma_prefetch_desc(&tmap_q); tma_prefetch_desc(&tmap_k); tma_prefetch_desc(&tmap_v);
     mbar_init(q_full, 1);
     for (int i = 0; i < 2; ++i) {
-      mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 2);   // one arrival per consumer warpgroup
-      mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], 2);
+      mbar_init(&k_full[i], KV8 ? 128 : 1); mbar_init(&k_empty[i], 2);   // one arrival per consumer warpgroup
+      mbar_init(&v_full[i], KV8 ? 128 : 1); mbar_init(&v_empty[i], 2);   // KV8: one per expanding producer thread
+      if (KV8) mbar_init(&c_full[i], 1);
     }
     fence_barrier_init();
   }
   __syncthreads();
 
+  if (KV8 && wg == 0) {
+    auto issue_codes = [&](int j) {   // thread 0: K and V codes of tile j into code stage j & 1
+      const int st = j & 1;
+      const int row0 = (pages[min(j, p.max_pages - 1)] * p.nkv + kvh) * kPageTokens;
+      mbar_arrive_expect_tx(&c_full[st], 2 * kTcTile8);
+      tma_load_2d(s8 + st * 2 * kTcTile8, &tmap_k, &c_full[st], 0, row0, kEvictLast);
+      tma_load_2d(s8 + st * 2 * kTcTile8 + kTcTile8, &tmap_v, &c_full[st], 0, row0, kEvictLast);
+    };
+    if (threadIdx.x == 0) {
+      mbar_arrive_expect_tx(q_full, 2 * kTcTile);
+      tma_load_2d(sQ, &tmap_q, q_full, h * kHeadDim, tok0 + q0, kEvictNormal);
+      tma_load_2d(sQ + kTcTile, &tmap_q, q_full, h * kHeadDim + 64, tok0 + q0, kEvictNormal);
+      for (int j = 0; j < min(2, ntiles); ++j) issue_codes(j);
+    }
+    for (int j = 0; j < ntiles; ++j) {
+      const int st = j & 1;
+      const uint32_t ph = (j >> 1) & 1;
+      const uint8_t* codes = s8 + st * 2 * kTcTile8;
+      mbar_wait(&c_full[st], ph);
+      mbar_wait(&k_empty[st], ph ^ 1);
+      expand_tc_tile8(sK + st * kTcTile, codes, kTcKv);   // K rows past kv_end are masked, whatever they hold
+      fence_proxy_async_shared();                          // generic-proxy stores -> visible to wgmma
+      mbar_arrive(&k_full[st]);
+      mbar_wait(&v_empty[st], ph ^ 1);
+      expand_tc_tile8(sV + st * kTcTile, codes + kTcTile8, kv_end - j * kTcKv);   // 0 * stale V row would be NaN
+      fence_proxy_async_shared();
+      mbar_arrive(&v_full[st]);
+      if (j + 2 < ntiles) {
+        asm volatile("bar.sync 2, 128;" ::: "memory");   // every producer thread is done reading code stage st
+        if (threadIdx.x == 0) issue_codes(j + 2);
+      }
+    }
+    return;
+  }
   if (wg == 0) {
     if (threadIdx.x == 0) {
       mbar_arrive_expect_tx(q_full, 2 * kTcTile);
@@ -167,7 +231,7 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
     for (int i = 0; i < 64; ++i) o[i] *= corr[(i >> 1) & 1];
     // ---- O += P V: 16 tokens per MMA; the S fragment of tokens [16k, 16k + 16) is the A fragment {pa[4k] .. pa[4k + 3]}
     mbar_wait(&v_full[st], ph);
-    if (kv_end < (j + 1) * kTcKv) {   // the tile straddling kv_end (uniform per CTA): zero its V rows past the end
+    if (!KV8 && kv_end < (j + 1) * kTcKv) {   // the tile straddling kv_end (uniform per CTA): zero its V rows past the end
       // a 128B-swizzled row keeps its 128 bytes, so row r of each [64 x 64] box is bytes [128 r, 128 r + 128)
       uint8_t* vd = sV + st * kTcTile;
       const int r0 = kv_end - j * kTcKv;

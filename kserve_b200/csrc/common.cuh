@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -53,6 +54,31 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
 __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
   __nv_bfloat162 v = *reinterpret_cast<__nv_bfloat162*>(&u);
   return __bfloat1622float2(v);
+}
+
+// FP8 KV cache codes: e4m3(clamp(x, -448, 448)), round to nearest even; NaN stays NaN.  `lo` goes to the lower byte.
+__device__ __forceinline__ uint32_t e4m3x2_rn_sat(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+// 8 bf16 (one 16-byte chunk) -> their 8 codes, byte i = element i
+__device__ __forceinline__ uint2 bf16x8_to_e4m3(const uint4& v) {
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+  uint32_t c[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float2 f = unpack_bf16x2(w[i]);
+    c[i] = e4m3x2_rn_sat(f.x, f.y);
+  }
+  return make_uint2(c[0] | (c[1] << 16), c[2] | (c[3] << 16));
+}
+// the value an FP8 KV cache gives back for x: float(e4m3(clamp(x))) (exact in bf16 and in half)
+__device__ __forceinline__ float e4m3_roundtrip(float x) {
+  const uint16_t c = (uint16_t)e4m3x2_rn_sat(x, 0.f);
+  uint32_t h2;
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h2) : "h"(c));
+  return __half2float(__ushort_as_half((unsigned short)(h2 & 0xFFFFu)));
 }
 
 // 128-bit streaming load that does not allocate in L1 (weights / KV pages are read once per step).

@@ -112,8 +112,9 @@ struct b200_engine {
   bool finalized = false;
   bf16 *cos_tab = nullptr, *sin_tab = nullptr;
   // KV cache
-  bf16 *kcache = nullptr, *vcache = nullptr;
-  long long layer_stride = 0;  // elements per layer in each cache
+  uint8_t *kcache = nullptr, *vcache = nullptr;   // bf16, or e4m3 codes when kv8
+  bool kv8 = false;            // cfg.kv_cache_dtype == 1
+  long long layer_stride = 0;  // bytes per layer in each cache
   int num_pages = 0, max_pages = 0;
   int32_t* d_page_table = nullptr;
   std::vector<int32_t> h_page_table;
@@ -366,8 +367,9 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
       w.wgu = w.wo + H_ * QH;
       w.wdown = w.wgu + 2 * I_ * H_;
     }
-    bf16* kc = e->kcache + (long long)l * e->layer_stride;
-    bf16* vc = e->vcache + (long long)l * e->layer_stride;
+    // (with an FP8 KV cache the kernels' bf16 cache pointers address e4m3 codes: the kv8 instantiations read them as such)
+    bf16* kc = reinterpret_cast<bf16*>(e->kcache + (long long)l * e->layer_stride);
+    bf16* vc = reinterpret_cast<bf16*>(e->vcache + (long long)l * e->layer_stride);
     // ---- QKV projection
     RopeKvParams rp{};
     bool fused_rope = false;
@@ -391,7 +393,7 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
       rp.q_out = e->qkv + r0 * e->qkv_cols; rp.ldq = e->qkv_cols;  // in place
       rp.tok_seq = e->d_tok_seq + r0; rp.tok_pos = e->d_tok_pos + r0;
       rp.kcache = kc; rp.vcache = vc; rp.page_table = e->d_page_table; rp.max_pages = e->max_pages;
-      rp.cos_tab = e->cos_tab; rp.sin_tab = e->sin_tab; rp.nh = e->nh; rp.nkv = e->nkv;
+      rp.cos_tab = e->cos_tab; rp.sin_tab = e->sin_tab; rp.nh = e->nh; rp.nkv = e->nkv; rp.kv8 = e->kv8;
       // RoPE + KV append in the QKV GEMM's epilogue (the separate rope_kv_kernel pass re-read and re-wrote 750 MB per layer
       // at 0.37 of the HBM peak); B200_NO_ROPE_FUSION=1 restores the two-kernel path
       static const bool rope_fused = getenv("B200_NO_ROPE_FUSION") == nullptr;
@@ -407,7 +409,9 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
     e->launches++;
     if (!decode && !fused_rope) {   // decode: RoPE + KV append are fused into attn_decode_kernel
       rp.T = T; rp.tokens_per_cta = 1;   // (4 tokens per CTA measured SLOWER: 446 vs 312 us per launch, r02 ncu)
-      B200_CUDA_OK(launch_k(rope_kv_kernel, dim3((T + rp.tokens_per_cta - 1) / rp.tokens_per_cta), dim3(512), 0, s, rp));
+      const dim3 grid((T + rp.tokens_per_cta - 1) / rp.tokens_per_cta);
+      if (e->kv8) B200_CUDA_OK(launch_k(rope_kv_kernel<true>, grid, dim3(512), 0, s, rp));
+      else B200_CUDA_OK(launch_k(rope_kv_kernel<false>, grid, dim3(512), 0, s, rp));
       e->launches++;
     }
     // ---- attention
@@ -429,7 +433,7 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
       ap.kcache_w = kc; ap.vcache_w = vc;
       static const bool fold = getenv("B200_ATTN_COMBINE_KERNEL") == nullptr;   // =1: separate attn_combine_kernel (A/B)
       ap.split_counter = fold ? e->attn_split_cnt : nullptr;
-      if ((rc = launch_attn_decode(ap, B, s))) return rc;
+      if ((rc = launch_attn_decode(ap, B, s, e->kv8))) return rc;
       e->launches += (ap.splits > 1 && !ap.split_counter) ? 2 : 1;
     } else {
       AttnPrefillParams ap{};
@@ -445,7 +449,8 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
         tp_.out = e->attn; tp_.ldo = e->nh * kHeadDim; tp_.page_table = e->d_page_table; tp_.max_pages = e->max_pages;
         tp_.cu_seqlens = e->d_cu + vw.b0; tp_.seq_slot = e->d_seq_slot + vw.b0; tp_.nh = e->nh; tp_.nkv = e->nkv; tp_.scale_log2 = scale_log2;
         tp_.kv_off = kv_off ? kv_off + vw.b0 : nullptr;
-        if ((rc = launch_attn_prefill_tc(e->tmaps, e->qkv, e->cap_T, e->qkv_cols, kc, vc, e->num_pages, tp_, B, max_len, s))) return rc;
+        if ((rc = launch_attn_prefill_tc(e->tmaps, e->qkv, e->cap_T, e->qkv_cols, kc, vc, e->num_pages, tp_, B, max_len, s, e->kv8)))
+          return rc;
       }
       e->launches++;
     }
@@ -1301,6 +1306,11 @@ int b200_engine_create(const b200_model_config_t* c, const void* nccl_id, b200_e
   B200_REQUIRE(c->weight_format == 0 || c->weight_format == 1, "weight_format must be 0 (bf16) or 1 (fp8 e4m3, a scale per row)");
   B200_REQUIRE(c->weight_format == 0 || c->num_experts == 0, "FP8 weights are supported for dense models only (no MoE experts)");
   B200_REQUIRE(c->weight_format == 0 || c->tp_size == 1, "FP8 weights are supported on one GPU only (tensor parallel tp_size > 1 is not)");
+  B200_REQUIRE(c->kv_cache_dtype == 0 || c->kv_cache_dtype == 1, "kv_cache_dtype must be 0 (bf16) or 1 (float8_e4m3fn)");
+  B200_REQUIRE(c->kv_cache_dtype == 0 || c->tp_size == 1,
+               "an FP8 KV cache is supported on one GPU only (tensor parallel tp_size > 1 is not)");
+  B200_REQUIRE(c->kv_cache_dtype == 0 || getenv("B200_ATTN_MMA") == nullptr,
+               "an FP8 KV cache needs the wgmma prefill attention (unset B200_ATTN_MMA)");
   int ndev = 0;
   B200_CUDA_OK(cudaGetDeviceCount(&ndev));
   B200_REQUIRE(c->device >= 0 && c->device < ndev, "no such CUDA device (this library has no CPU fallback)");
@@ -1388,14 +1398,15 @@ int b200_engine_create(const b200_model_config_t* c, const void* nccl_id, b200_e
     B200_CUDA_OK(cudaMemcpy(e->cos_tab, hc.data(), hc.size() * 2, cudaMemcpyHostToDevice));
     B200_CUDA_OK(cudaMemcpy(e->sin_tab, hs.data(), hs.size() * 2, cudaMemcpyHostToDevice));
   }
-  // KV cache (zero-filled: masked-out V rows must be finite)
+  // KV cache (zero-filled: masked-out V rows must be finite); bf16, or one e4m3 code per element
+  e->kv8 = c->kv_cache_dtype == 1;
   e->max_pages = (c->max_seq_len + kPageTokens - 1) / kPageTokens;
   e->num_pages = c->num_kv_pages > 0 ? c->num_kv_pages : c->max_batch * e->max_pages;
-  e->layer_stride = (long long)e->num_pages * e->nkv * kPageTokens * kHeadDim;
+  e->layer_stride = (long long)e->num_pages * e->nkv * kPageTokens * kHeadDim * (e->kv8 ? 1 : (long long)sizeof(bf16));
   if ((rc = dmalloc(&e->kcache, (size_t)e->layer_stride * e->L))) return rc;
   if ((rc = dmalloc(&e->vcache, (size_t)e->layer_stride * e->L))) return rc;
-  B200_CUDA_OK(cudaMemset(e->kcache, 0, (size_t)e->layer_stride * e->L * 2));
-  B200_CUDA_OK(cudaMemset(e->vcache, 0, (size_t)e->layer_stride * e->L * 2));
+  B200_CUDA_OK(cudaMemset(e->kcache, 0, (size_t)e->layer_stride * e->L));
+  B200_CUDA_OK(cudaMemset(e->vcache, 0, (size_t)e->layer_stride * e->L));
   if ((rc = dmalloc(&e->d_page_table, (size_t)c->max_batch * e->max_pages))) return rc;
   e->h_page_table.assign((size_t)c->max_batch * e->max_pages, 0);
   // activations
@@ -1964,9 +1975,9 @@ static int kv_swap(b200_engine_t* e, int32_t slot, bool out, int scrub) {
   auto& st = e->st;
   B200_REQUIRE(st.prefilled && slot >= 0 && slot < st.B, "no such staged sequence");
   B200_CUDA_OK(cudaSetDevice(e->cfg.device));
-  const size_t page_elems = (size_t)e->nkv * kPageTokens * kHeadDim;
-  const size_t seq_elems = (size_t)st.per_seq_pages * page_elems;          // per layer, per K or V
-  const size_t bytes = seq_elems * 2 * 2 * e->L;
+  const size_t page_bytes = (size_t)e->nkv * kPageTokens * kHeadDim * (e->kv8 ? 1 : sizeof(bf16));
+  const size_t seq_bytes = (size_t)st.per_seq_pages * page_bytes;         // per layer, per K or V
+  const size_t bytes = seq_bytes * 2 * e->L;
   if (out) {
     if (!e->host_kv.count(slot) || e->host_kv_bytes[slot] < bytes) {
       if (e->host_kv.count(slot)) cudaFreeHost(e->host_kv[slot]);
@@ -1977,23 +1988,23 @@ static int kv_swap(b200_engine_t* e, int32_t slot, bool out, int scrub) {
   } else {
     B200_REQUIRE(e->host_kv.count(slot), "sequence is not swapped out");
   }
-  bf16* h = e->host_kv[slot];
-  const size_t first = (size_t)slot * st.per_seq_pages * page_elems;
+  unsigned char* h = reinterpret_cast<unsigned char*>(e->host_kv[slot]);
+  const size_t first = (size_t)slot * seq_bytes;
   for (int l = 0; l < e->L; ++l) {
-    bf16* kd = e->kcache + (size_t)l * e->layer_stride + first;
-    bf16* vd = e->vcache + (size_t)l * e->layer_stride + first;
-    bf16* kh = h + ((size_t)l * 2) * seq_elems;
-    bf16* vh = kh + seq_elems;
+    uint8_t* kd = e->kcache + (size_t)l * e->layer_stride + first;
+    uint8_t* vd = e->vcache + (size_t)l * e->layer_stride + first;
+    unsigned char* kh = h + ((size_t)l * 2) * seq_bytes;
+    unsigned char* vh = kh + seq_bytes;
     if (out) {
-      B200_CUDA_OK(cudaMemcpyAsync(kh, kd, seq_elems * 2, cudaMemcpyDeviceToHost, e->stream));
-      B200_CUDA_OK(cudaMemcpyAsync(vh, vd, seq_elems * 2, cudaMemcpyDeviceToHost, e->stream));
+      B200_CUDA_OK(cudaMemcpyAsync(kh, kd, seq_bytes, cudaMemcpyDeviceToHost, e->stream));
+      B200_CUDA_OK(cudaMemcpyAsync(vh, vd, seq_bytes, cudaMemcpyDeviceToHost, e->stream));
       if (scrub) {
-        B200_CUDA_OK(cudaMemsetAsync(kd, 0x7f, seq_elems * 2, e->stream));
-        B200_CUDA_OK(cudaMemsetAsync(vd, 0x7f, seq_elems * 2, e->stream));
+        B200_CUDA_OK(cudaMemsetAsync(kd, 0x7f, seq_bytes, e->stream));
+        B200_CUDA_OK(cudaMemsetAsync(vd, 0x7f, seq_bytes, e->stream));
       }
     } else {
-      B200_CUDA_OK(cudaMemcpyAsync(kd, kh, seq_elems * 2, cudaMemcpyHostToDevice, e->stream));
-      B200_CUDA_OK(cudaMemcpyAsync(vd, vh, seq_elems * 2, cudaMemcpyHostToDevice, e->stream));
+      B200_CUDA_OK(cudaMemcpyAsync(kd, kh, seq_bytes, cudaMemcpyHostToDevice, e->stream));
+      B200_CUDA_OK(cudaMemcpyAsync(vd, vh, seq_bytes, cudaMemcpyHostToDevice, e->stream));
     }
   }
   return 0;
@@ -2134,8 +2145,7 @@ static int cb_swap(b200_engine_t* e, int32_t slot, bool out) {
   B200_REQUIRE(e && e->cb_on, "not in continuous-batching mode");
   B200_REQUIRE(slot >= 0 && slot < e->cfg.max_batch && e->cb_used[slot], "slot is not in use");
   B200_CUDA_OK(cudaSetDevice(e->cfg.device));
-  const size_t page_elems = (size_t)e->nkv * kPageTokens * kHeadDim;      // per layer, per K or V
-  const size_t page_bytes = page_elems * sizeof(bf16);
+  const size_t page_bytes = (size_t)e->nkv * kPageTokens * kHeadDim * (e->kv8 ? 1 : sizeof(bf16));   // per layer, per K or V
   cudaStream_t s = e->stream;
   if (out) {
     B200_REQUIRE(!e->cb_swapped[slot], "sequence is already swapped out");
@@ -2152,10 +2162,10 @@ static int cb_swap(b200_engine_t* e, int32_t slot, bool out) {
     unsigned char* h = reinterpret_cast<unsigned char*>(e->host_kv[slot]);
     for (size_t i = 0; i < pages.size(); ++i) {     // one strided copy per page and cache: [L] rows of page_bytes
       unsigned char* hk = h + (i * 2) * page_bytes * e->L;
-      B200_CUDA_OK(cudaMemcpy2DAsync(hk, page_bytes, e->kcache + (size_t)pages[i] * page_elems, (size_t)e->layer_stride * sizeof(bf16),
+      B200_CUDA_OK(cudaMemcpy2DAsync(hk, page_bytes, e->kcache + (size_t)pages[i] * page_bytes, (size_t)e->layer_stride,
                                      page_bytes, e->L, cudaMemcpyDeviceToHost, s));
-      B200_CUDA_OK(cudaMemcpy2DAsync(hk + page_bytes * e->L, page_bytes, e->vcache + (size_t)pages[i] * page_elems,
-                                     (size_t)e->layer_stride * sizeof(bf16), page_bytes, e->L, cudaMemcpyDeviceToHost, s));
+      B200_CUDA_OK(cudaMemcpy2DAsync(hk + page_bytes * e->L, page_bytes, e->vcache + (size_t)pages[i] * page_bytes,
+                                     (size_t)e->layer_stride, page_bytes, e->L, cudaMemcpyDeviceToHost, s));
     }
     e->cb_swap_pages[slot] = (int)pages.size();
     for (int pg : pages) cb_unref_page(e, pg);       // reuse is stream-ordered after the copies above
@@ -2181,9 +2191,9 @@ static int cb_swap(b200_engine_t* e, int32_t slot, bool out) {
   const unsigned char* h = reinterpret_cast<const unsigned char*>(e->host_kv[slot]);
   for (int i = 0; i < n; ++i) {
     const unsigned char* hk = h + ((size_t)i * 2) * page_bytes * e->L;
-    B200_CUDA_OK(cudaMemcpy2DAsync(e->kcache + (size_t)got[i] * page_elems, (size_t)e->layer_stride * sizeof(bf16), hk, page_bytes,
+    B200_CUDA_OK(cudaMemcpy2DAsync(e->kcache + (size_t)got[i] * page_bytes, (size_t)e->layer_stride, hk, page_bytes,
                                    page_bytes, e->L, cudaMemcpyHostToDevice, s));
-    B200_CUDA_OK(cudaMemcpy2DAsync(e->vcache + (size_t)got[i] * page_elems, (size_t)e->layer_stride * sizeof(bf16), hk + page_bytes * e->L,
+    B200_CUDA_OK(cudaMemcpy2DAsync(e->vcache + (size_t)got[i] * page_bytes, (size_t)e->layer_stride, hk + page_bytes * e->L,
                                    page_bytes, page_bytes, e->L, cudaMemcpyHostToDevice, s));
   }
   e->cb_slot_pages[slot] = got;
@@ -2349,17 +2359,34 @@ int b200_op_attn_prefill(const void* q, int64_t ldq, void* out, int64_t ldo, con
   return launch_attn_prefill(p, B, max_len, (cudaStream_t)stream);
 }
 
-int b200_op_attn_prefill_tc_off(const void* q, int64_t ldq, int q_rows, void* out, int64_t ldo, const void* kcache,
-                                const void* vcache, int num_pages, const int32_t* page_table, int max_pages,
-                                const int32_t* cu_seqlens, const int32_t* seq_slot, const int32_t* kv_off, int B, int max_len,
-                                int nh, int nkv, void* stream) {
+static int op_attn_prefill_tc(const void* q, int64_t ldq, int q_rows, void* out, int64_t ldo, const void* kcache,
+                              const void* vcache, int num_pages, const int32_t* page_table, int max_pages,
+                              const int32_t* cu_seqlens, const int32_t* seq_slot, const int32_t* kv_off, int B, int max_len,
+                              int nh, int nkv, void* stream, bool kv8) {
   g_op_tmaps.maps.clear();
+  g_op_tmaps.maps_kv8.clear();
   AttnTcParams p{};
   p.out = (bf16*)out; p.ldo = ldo; p.page_table = page_table; p.max_pages = max_pages; p.cu_seqlens = cu_seqlens;
   p.seq_slot = seq_slot; p.nh = nh; p.nkv = nkv; p.scale_log2 = (1.0f / sqrtf((float)kHeadDim)) * 1.4426950408889634f;
   p.kv_off = kv_off;
-  return launch_attn_prefill_tc(g_op_tmaps, (const bf16*)q, q_rows, ldq, (const bf16*)kcache, (const bf16*)vcache, num_pages, p, B,
-                                max_len, (cudaStream_t)stream);
+  return launch_attn_prefill_tc(g_op_tmaps, (const bf16*)q, q_rows, ldq, kcache, vcache, num_pages, p, B, max_len,
+                                (cudaStream_t)stream, kv8);
+}
+
+int b200_op_attn_prefill_tc_off(const void* q, int64_t ldq, int q_rows, void* out, int64_t ldo, const void* kcache,
+                                const void* vcache, int num_pages, const int32_t* page_table, int max_pages,
+                                const int32_t* cu_seqlens, const int32_t* seq_slot, const int32_t* kv_off, int B, int max_len,
+                                int nh, int nkv, void* stream) {
+  return op_attn_prefill_tc(q, ldq, q_rows, out, ldo, kcache, vcache, num_pages, page_table, max_pages, cu_seqlens, seq_slot,
+                            kv_off, B, max_len, nh, nkv, stream, false);
+}
+
+int b200_op_attn_prefill_tc_kv8(const void* q, int64_t ldq, int q_rows, void* out, int64_t ldo, const void* kcache,
+                                const void* vcache, int num_pages, const int32_t* page_table, int max_pages,
+                                const int32_t* cu_seqlens, const int32_t* seq_slot, const int32_t* kv_off, int B, int max_len,
+                                int nh, int nkv, void* stream) {
+  return op_attn_prefill_tc(q, ldq, q_rows, out, ldo, kcache, vcache, num_pages, page_table, max_pages, cu_seqlens, seq_slot,
+                            kv_off, B, max_len, nh, nkv, stream, true);
 }
 
 int b200_op_attn_prefill_tc(const void* q, int64_t ldq, int q_rows, void* out, int64_t ldo, const void* kcache,
@@ -2381,11 +2408,11 @@ int b200_op_attn_decode(const void* q, int64_t ldq, void* out, int64_t ldo, cons
   return launch_attn_decode(p, B, (cudaStream_t)stream);
 }
 
-int b200_op_attn_decode_fused(const void* qkv, int64_t ld_qkv, const float* qkv_partial, int qkv_splits, int64_t split_stride,
-                              int64_t ld_partial, const void* qkv_bias, const void* cos_tab, const void* sin_tab, void* out,
-                              int64_t ldo, void* kcache, void* vcache, const int32_t* page_table, int max_pages,
-                              const int32_t* seq_slot, const int32_t* tok_pos, int B, int nh, int nkv, int splits, float* part_o,
-                              float* part_ml, int32_t* split_counter, void* stream) {
+static int op_attn_decode_fused(const void* qkv, int64_t ld_qkv, const float* qkv_partial, int qkv_splits, int64_t split_stride,
+                                int64_t ld_partial, const void* qkv_bias, const void* cos_tab, const void* sin_tab, void* out,
+                                int64_t ldo, void* kcache, void* vcache, const int32_t* page_table, int max_pages,
+                                const int32_t* seq_slot, const int32_t* tok_pos, int B, int nh, int nkv, int splits, float* part_o,
+                                float* part_ml, int32_t* split_counter, void* stream, bool kv8) {
   B200_REQUIRE((qkv == nullptr) != (qkv_partial == nullptr), "exactly one of qkv / qkv_partial must be given");
   B200_REQUIRE(qkv_bias == nullptr || qkv_partial != nullptr, "qkv_bias applies to split-K partials only");
   AttnDecodeParams p{};
@@ -2398,7 +2425,28 @@ int b200_op_attn_decode_fused(const void* qkv, int64_t ld_qkv, const float* qkv_
   p.qkv_bias = (const bf16*)qkv_bias; p.cos_tab = (const bf16*)cos_tab; p.sin_tab = (const bf16*)sin_tab;
   p.kcache_w = (bf16*)kcache; p.vcache_w = (bf16*)vcache;
   p.split_counter = split_counter;
-  return launch_attn_decode(p, B, (cudaStream_t)stream);
+  return launch_attn_decode(p, B, (cudaStream_t)stream, kv8);
+}
+
+int b200_op_attn_decode_fused(const void* qkv, int64_t ld_qkv, const float* qkv_partial, int qkv_splits, int64_t split_stride,
+                              int64_t ld_partial, const void* qkv_bias, const void* cos_tab, const void* sin_tab, void* out,
+                              int64_t ldo, void* kcache, void* vcache, const int32_t* page_table, int max_pages,
+                              const int32_t* seq_slot, const int32_t* tok_pos, int B, int nh, int nkv, int splits, float* part_o,
+                              float* part_ml, int32_t* split_counter, void* stream) {
+  return op_attn_decode_fused(qkv, ld_qkv, qkv_partial, qkv_splits, split_stride, ld_partial, qkv_bias, cos_tab, sin_tab, out, ldo,
+                              kcache, vcache, page_table, max_pages, seq_slot, tok_pos, B, nh, nkv, splits, part_o, part_ml,
+                              split_counter, stream, false);
+}
+
+int b200_op_attn_decode_fused_kv8(const void* qkv, int64_t ld_qkv, const float* qkv_partial, int qkv_splits,
+                                  int64_t split_stride, int64_t ld_partial, const void* qkv_bias, const void* cos_tab,
+                                  const void* sin_tab, void* out, int64_t ldo, void* kcache, void* vcache,
+                                  const int32_t* page_table, int max_pages, const int32_t* seq_slot, const int32_t* tok_pos,
+                                  int B, int nh, int nkv, int splits, float* part_o, float* part_ml, int32_t* split_counter,
+                                  void* stream) {
+  return op_attn_decode_fused(qkv, ld_qkv, qkv_partial, qkv_splits, split_stride, ld_partial, qkv_bias, cos_tab, sin_tab, out, ldo,
+                              kcache, vcache, page_table, max_pages, seq_slot, tok_pos, B, nh, nkv, splits, part_o, part_ml,
+                              split_counter, stream, true);
 }
 
 int b200_op_rope_kv(const void* qkv, int64_t ld, void* q_out, int64_t ldq, void* kcache, void* vcache,
@@ -2409,7 +2457,7 @@ int b200_op_rope_kv(const void* qkv, int64_t ld, void* q_out, int64_t ldq, void*
   p.page_table = page_table; p.max_pages = max_pages; p.tok_seq = tok_seq; p.tok_pos = tok_pos;
   p.cos_tab = (const bf16*)cos_tab; p.sin_tab = (const bf16*)sin_tab; p.nh = nh; p.nkv = nkv;
   p.T = T; p.tokens_per_cta = (getenv("B200_ROPE_TOKENS_PER_CTA") && T >= 4096) ? atoi(getenv("B200_ROPE_TOKENS_PER_CTA")) : 1;
-  rope_kv_kernel<<<(T + p.tokens_per_cta - 1) / p.tokens_per_cta, 512, 0, (cudaStream_t)stream>>>(p);
+  rope_kv_kernel<false><<<(T + p.tokens_per_cta - 1) / p.tokens_per_cta, 512, 0, (cudaStream_t)stream>>>(p);
   B200_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -62,12 +62,14 @@ __device__ __forceinline__ float2 ld_bias2(const bf16* b, int col, int N) {
 // tmap_out: `out` as [rows][out columns] with leading dimension ldo, box [128][64], 128B swizzle; used when p.out_tma.
 // BIAS (EPI_STORE, EPI_ROPE_KV): add p.bias[column] to the fp32 accumulator before its bf16 rounding; a compile-time
 // flag, so the GEMMs without a bias run exactly the code they ran before.
-template <int EPI, bool BIAS = false>
+// KV8 (EPI_ROPE_KV): the paged cache holds e4m3 codes; each k / v row goes out as e4m3(bf16 value), 8 codes per store.
+template <int EPI, bool BIAS = false, bool KV8 = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_prefill_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                     const __grid_constant__ CUtensorMap tmap_out, const GemmParams p) {
   static_assert(EPI == EPI_STORE || EPI == EPI_STORE_RES || EPI == EPI_SWIGLU || EPI == EPI_ROPE_KV, "row-major epilogues only");
   static_assert(!BIAS || EPI == EPI_STORE || EPI == EPI_ROPE_KV, "bias: QKV epilogues only");
+  static_assert(!KV8 || EPI == EPI_ROPE_KV, "FP8 KV cache: the RoPE + KV epilogue only");
   TraceScope _ts(TK_GEMM + 100 * EPI + 1000 * (p.M >> 7));
   using Cfg = PrefillCfg<EPI>;
   constexpr int STAGES = Cfg::kStages;
@@ -289,6 +291,7 @@ gemm_prefill_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
       const int r = et & (kGemmBlockM - 1), hsel = et >> 7;
       const int m = row0 + r;
       bf16* dst = nullptr;
+      uint8_t* dst8 = nullptr;   // KV8: this row's k / v codes
       int nvalid = HC;
       bool vec = out_vec;
       int stream = p.stream_out;
@@ -301,8 +304,14 @@ gemm_prefill_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
             const int pos = p.rope_tok_pos[m + roff];
             const int page = p.rope_page_table[(long long)p.rope_tok_seq[m + roff] * p.rope_max_pages + (pos >> 6)];
             const long long page_row = (long long)page * p.rope_nkv * 64 + (pos & 63);   // row of kv head 0 in [..][64][128]
-            dst = head < p.rope_nh + p.rope_nkv ? p.rope_kcache + (page_row + (long long)(head - p.rope_nh) * 64) * 128
-                                                : p.rope_vcache + (page_row + (long long)(head - p.rope_nh - p.rope_nkv) * 64) * 128;
+            if constexpr (KV8) {
+              const long long e0 = head < p.rope_nh + p.rope_nkv ? (page_row + (long long)(head - p.rope_nh) * 64) * 128
+                                                                 : (page_row + (long long)(head - p.rope_nh - p.rope_nkv) * 64) * 128;
+              dst8 = reinterpret_cast<uint8_t*>(head < p.rope_nh + p.rope_nkv ? p.rope_kcache : p.rope_vcache) + e0;
+            } else {
+              dst = head < p.rope_nh + p.rope_nkv ? p.rope_kcache + (page_row + (long long)(head - p.rope_nh) * 64) * 128
+                                                  : p.rope_vcache + (page_row + (long long)(head - p.rope_nh - p.rope_nkv) * 64) * 128;
+            }
             vec = true;
             stream = 0;
           }
@@ -310,6 +319,13 @@ gemm_prefill_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
           const int ncols = (EPI == EPI_SWIGLU) ? p.out_cols : p.N;
           nvalid = min(HC, ncols - (oc0 + HC * hsel));
           if (nvalid > 0) dst = reinterpret_cast<bf16*>(p.out) + (long long)(m + roff) * p.ldo + oc0 + HC * hsel;
+        }
+      }
+      if constexpr (KV8) {
+        if (dst8 != nullptr) {
+#pragma unroll 4
+          for (int c = 0; c < HC; c += 8)
+            *reinterpret_cast<uint2*>(dst8 + c) = bf16x8_to_e4m3(ld_shared_v4(ot + out_tile_off(r, HC * hsel + c)));
         }
       }
       if (dst != nullptr) {

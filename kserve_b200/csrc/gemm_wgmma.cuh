@@ -60,7 +60,7 @@ struct GemmParams {
   // EPI_ROPE_KV: one output row = one prompt token (HF bf16 rounding points of apply_rotary_pos_emb; bit-identical to rope_kv_kernel)
   const int32_t* rope_tok_seq; const int32_t* rope_tok_pos;   // [M] page-table row / position of each token
   const int32_t* rope_page_table; int rope_max_pages;
-  bf16* rope_kcache; bf16* rope_vcache;                      // this layer's [page][kv_head][64][128]
+  bf16* rope_kcache; bf16* rope_vcache;                      // this layer's [page][kv_head][64][128] (KV8: e4m3 codes)
   const bf16* rope_cos; const bf16* rope_sin;                // [max_pos][64]
   int rope_nh, rope_nkv;
   int stream_out;          // row-major epilogues: cache-streaming output stores

@@ -59,14 +59,15 @@ inline int make_tmap_2d(CUtensorMap* map, const void* ptr, uint64_t rows, uint64
   return 0;
 }
 
-// 2D e4m3 codes [rows][cols] (FP8 weights), box = [box_rows][64 bytes], unswizzled, OOB -> zeros.
-inline int make_tmap_2d_u8(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+// 2D e4m3 codes [rows][cols] (FP8 weights, FP8 KV cache), box = [box_rows][box_cols bytes], unswizzled, OOB -> zeros.
+inline int make_tmap_2d_u8(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows,
+                           uint32_t box_cols = 64) {
   PFN_encodeTiled fn = get_encode_fn();
   B200_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled entry point not available (no CUDA driver?)");
   B200_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && cols % 16 == 0, "FP8 TMA: 16-byte aligned base and rows");
   cuuint64_t dims[2] = {cols, rows};
   cuuint64_t strides[1] = {cols};
-  cuuint32_t box[2] = {64, box_rows};
+  cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), dims, strides, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -78,6 +79,19 @@ inline int make_tmap_2d_u8(CUtensorMap* map, const void* ptr, uint64_t rows, uin
 struct TmapCache {
   std::map<std::tuple<const void*, uint64_t, uint64_t, uint32_t, uint64_t>, CUtensorMap> maps;
   std::map<std::tuple<const void*, uint64_t, uint64_t>, CUtensorMap> maps_u8;   // FP8 weights, 128-row boxes
+  std::map<std::pair<const void*, uint64_t>, CUtensorMap> maps_kv8;               // FP8 KV caches, one 64 x 128 B tile a box
+  int get_kv8(const void* ptr, uint64_t rows, const CUtensorMap** out) {
+    auto key = std::make_pair(ptr, rows);
+    auto it = maps_kv8.find(key);
+    if (it == maps_kv8.end()) {
+      CUtensorMap m;
+      int rc = make_tmap_2d_u8(&m, ptr, rows, kHeadDim, kPageTokens, kHeadDim);
+      if (rc) return rc;
+      it = maps_kv8.emplace(key, m).first;
+    }
+    *out = &it->second;
+    return 0;
+  }
   int get_u8(const void* ptr, uint64_t rows, uint64_t cols, const CUtensorMap** out) {
     auto key = std::make_tuple(ptr, rows, cols);
     auto it = maps_u8.find(key);
@@ -137,10 +151,10 @@ inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_
   return cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
 }
 
-template <int EPI, bool BIAS = false>
+template <int EPI, bool BIAS = false, bool KV8 = false>
 int launch_prefill_inst(const CUtensorMap* ta, const CUtensorMap* tb, const CUtensorMap* to, const GemmParams& p, int grid,
                         cudaStream_t s) {
-  auto kern = gemm_prefill_kernel<EPI, BIAS>;
+  auto kern = gemm_prefill_kernel<EPI, BIAS, KV8>;
   static bool configured = false;  // per instantiation
   if (!configured) {
     B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PrefillCfg<EPI>::kSmemBytes));
@@ -307,6 +321,8 @@ inline int launch_gemm(TmapCache& cache, const GemmArgs& a, int num_sms, cudaStr
                                           : launch_prefill_inst<EPI_STORE>(ta, tb, to, p, grid, s);
     if (a.epi == EPI_STORE_RES) return launch_prefill_inst<EPI_STORE_RES>(ta, tb, to, p, grid, s);
     if (a.epi == EPI_SWIGLU) return launch_prefill_inst<EPI_SWIGLU>(ta, tb, to, p, grid, s);
+    if (a.rope->kv8) return a.bias ? launch_prefill_inst<EPI_ROPE_KV, true, true>(ta, tb, to, p, grid, s)
+                                   : launch_prefill_inst<EPI_ROPE_KV, false, true>(ta, tb, to, p, grid, s);
     return a.bias ? launch_prefill_inst<EPI_ROPE_KV, true>(ta, tb, to, p, grid, s)
                   : launch_prefill_inst<EPI_ROPE_KV>(ta, tb, to, p, grid, s);
   }
@@ -371,6 +387,7 @@ inline int launch_rmsnorm(int mode, bf16* x, const bf16* w, bf16* xn, int rows, 
 
 constexpr int kPrefillSmem = 5 * kTileBytes;
 constexpr int kDecodeSmem = 4096 + 2 * kDecStages * kTileBytes + 10 * kHeadDim * 4 + 2 * kHeadDim * 2;
+static_assert(2 * kTileBytes + kDecStages8 * 2 * kTile8Bytes == 2 * kDecStages * kTileBytes, "FP8 KV decode: same shared-memory layout");
 
 inline int launch_attn_prefill(const AttnPrefillParams& p, int B, int max_len, cudaStream_t s) {
   static bool configured = false;
@@ -383,34 +400,46 @@ inline int launch_attn_prefill(const AttnPrefillParams& p, int B, int max_len, c
   return 0;
 }
 
-// wgmma prefill attention: q rows [q_rows][ldq] (head h at column h*128), paged caches [num_pages][nkv][64][128]
-inline int launch_attn_prefill_tc(TmapCache& cache, const bf16* q, int q_rows, long long ldq, const bf16* kcache,
-                                  const bf16* vcache, int num_pages, const AttnTcParams& p, int B, int max_len, cudaStream_t s) {
+// wgmma prefill attention: q rows [q_rows][ldq] (head h at column h*128), paged caches [num_pages][nkv][64][128] of bf16,
+// or of e4m3 codes when kv8
+inline int launch_attn_prefill_tc(TmapCache& cache, const bf16* q, int q_rows, long long ldq, const void* kcache,
+                                  const void* vcache, int num_pages, const AttnTcParams& p, int B, int max_len, cudaStream_t s,
+                                  bool kv8 = false) {
   static bool configured = false;
   if (!configured) {
-    B200_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmem));
+    B200_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmem));
+    B200_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmem8));
     configured = true;
   }
   const CUtensorMap *tq, *tk, *tv;
   int rc = cache.get(q, (uint64_t)q_rows, (uint64_t)ldq, 128, &tq);
   if (rc) return rc;
   const uint64_t kv_rows = (uint64_t)num_pages * p.nkv * kPageTokens;
+  dim3 grid((max_len + kTcQ - 1) / kTcQ, p.nh, B);
+  if (kv8) {
+    if ((rc = cache.get_kv8(kcache, kv_rows, &tk))) return rc;
+    if ((rc = cache.get_kv8(vcache, kv_rows, &tv))) return rc;
+    B200_CUDA_OK(launch_k(attn_prefill_tc_kernel<true>, grid, dim3(kTcThreads), kTcSmem8, s, *tq, *tk, *tv, p));
+    return 0;
+  }
   if ((rc = cache.get(kcache, kv_rows, kHeadDim, 64, &tk))) return rc;
   if ((rc = cache.get(vcache, kv_rows, kHeadDim, 64, &tv))) return rc;
-  dim3 grid((max_len + kTcQ - 1) / kTcQ, p.nh, B);
-  B200_CUDA_OK(launch_k(attn_prefill_tc_kernel, grid, dim3(kTcThreads), kTcSmem, s, *tq, *tk, *tv, p));
+  B200_CUDA_OK(launch_k(attn_prefill_tc_kernel<false>, grid, dim3(kTcThreads), kTcSmem, s, *tq, *tk, *tv, p));
   return 0;
 }
 
-inline int launch_attn_decode(const AttnDecodeParams& p, int B, cudaStream_t s) {
+// kv8: the caches of `p` hold e4m3 codes (attn_decode_kernel<true>)
+inline int launch_attn_decode(const AttnDecodeParams& p, int B, cudaStream_t s, bool kv8 = false) {
   static bool configured = false;
   if (!configured) {
-    B200_CUDA_OK(cudaFuncSetAttribute(attn_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecodeSmem));
+    B200_CUDA_OK(cudaFuncSetAttribute(attn_decode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecodeSmem));
+    B200_CUDA_OK(cudaFuncSetAttribute(attn_decode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecodeSmem));
     configured = true;
   }
   B200_REQUIRE(p.G >= 1 && p.G <= 8, "GQA group size must be in [1, 8]");
   dim3 grid(B * p.nkv, p.splits);
-  B200_CUDA_OK(launch_k(attn_decode_kernel, grid, dim3(kAttnThreads), kDecodeSmem, s, p));
+  if (kv8) B200_CUDA_OK(launch_k(attn_decode_kernel<true>, grid, dim3(kAttnThreads), kDecodeSmem, s, p));
+  else B200_CUDA_OK(launch_k(attn_decode_kernel<false>, grid, dim3(kAttnThreads), kDecodeSmem, s, p));
   if (p.splits > 1 && !p.split_counter) {
     B200_CUDA_OK(launch_k(attn_combine_kernel, dim3(B * p.nh), dim3(128), 0, s, (const float*)p.part_o, (const float*)p.part_ml, p.out, p.ldo, p.nkv, p.G, p.splits));
   }

@@ -256,13 +256,14 @@ struct RopeKvParams {
   const bf16* qkv; long long ld;
   const float* partial; int splits; long long split_stride; long long ld_partial;
   bf16* q_out; long long ldq;
-  bf16* kcache; bf16* vcache;            // this layer's base
+  bf16* kcache; bf16* vcache;            // this layer's base (e4m3 codes in rope_kv_kernel<true>)
   const int32_t* page_table; int max_pages;  // [seq][max_pages]
   const int32_t* tok_seq;                // [T] sequence slot of each token
   const int32_t* tok_pos;                // [T] position within the sequence
   const bf16* cos_tab; const bf16* sin_tab;  // [max_pos][64]
   int nh, nkv;
   int T, tokens_per_cta;                     // tokens in this launch; consecutive tokens handled by one CTA
+  bool kv8;                                  // the caches hold e4m3 codes (rope_kv_kernel<true>, EPI_ROPE_KV's KV8 instantiation)
 };
 
 __device__ __forceinline__ void load8(const RopeKvParams& p, int t, int col, float (&f)[8]) {
@@ -289,6 +290,8 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
   return o;
 }
 
+// KV8: the cache holds e4m3 codes; k and v are stored as e4m3(bf16 value)
+template <bool KV8>
 __global__ void __launch_bounds__(512) rope_kv_kernel(const RopeKvParams p) {
   TraceScope _ts(TK_ROPE);
   pdl_launch_dependents();
@@ -333,17 +336,25 @@ __global__ void __launch_bounds__(512) rope_kv_kernel(const RopeKvParams p) {
         *reinterpret_cast<uint4*>(q + c + 64) = pack8(o2);
       } else {
         const int kvh = head - p.nh;
-        bf16* k = p.kcache + ((long long)page * p.nkv + kvh) * (kPageTokens * kHeadDim) + slot * kHeadDim;
-        *reinterpret_cast<uint4*>(k + c) = pack8(o1);
-        *reinterpret_cast<uint4*>(k + c + 64) = pack8(o2);
+        const long long e0 = ((long long)page * p.nkv + kvh) * (kPageTokens * kHeadDim) + slot * kHeadDim;
+        if constexpr (KV8) {
+          uint8_t* k = reinterpret_cast<uint8_t*>(p.kcache) + e0;
+          *reinterpret_cast<uint2*>(k + c) = bf16x8_to_e4m3(pack8(o1));
+          *reinterpret_cast<uint2*>(k + c + 64) = bf16x8_to_e4m3(pack8(o2));
+        } else {
+          bf16* k = p.kcache + e0;
+          *reinterpret_cast<uint4*>(k + c) = pack8(o1);
+          *reinterpret_cast<uint4*>(k + c + 64) = pack8(o2);
+        }
       }
     } else {
       const int j = it - rope_items;
       const int kvh = j >> 4, c = (j & 15) * 8;
       float f[8];
       load8(p, t, (p.nh + p.nkv + kvh) * kHeadDim + c, f);
-      bf16* v = p.vcache + ((long long)page * p.nkv + kvh) * (kPageTokens * kHeadDim) + slot * kHeadDim;
-      *reinterpret_cast<uint4*>(v + c) = pack8(f);
+      const long long e0 = ((long long)page * p.nkv + kvh) * (kPageTokens * kHeadDim) + slot * kHeadDim;
+      if constexpr (KV8) *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(p.vcache) + e0 + c) = bf16x8_to_e4m3(pack8(f));
+      else *reinterpret_cast<uint4*>(p.vcache + e0 + c) = pack8(f);
     }
   }
   }

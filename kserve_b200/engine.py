@@ -43,8 +43,9 @@ class B200Engine:
     def __init__(self, cfg: dict, *, max_batch: int = 8, max_seq_len: int = 2048,
                  max_prefill_tokens: Optional[int] = None, num_kv_pages: int = 0, device: int = 0,
                  tp_rank: int = 0, tp_size: int = 1, nccl_id: Optional[bytes] = None,
-                 vocab_rows: Optional[int] = None, weight_format: int = 0):
-        """weight_format 1: the seven projection weights are FP8 (float8_e4m3fn + a scale per row, kserve_b200/fp8.py)"""
+                 vocab_rows: Optional[int] = None, weight_format: int = 0, kv_cache_dtype: int = 0):
+        """weight_format 1: the seven projection weights are FP8 (float8_e4m3fn + a scale per row, kserve_b200/fp8.py);
+        kv_cache_dtype 1: the KV pages hold float8_e4m3fn codes (fp8.quantize_kv) instead of bf16"""
         self.lib = _lib.load()
         if not torch.cuda.is_available():
             raise _lib.B200Error("no CUDA device: kserve_b200 has no CPU fallback")
@@ -72,6 +73,8 @@ class B200Engine:
         mc.num_experts_per_tok = int(cfg.get("num_experts_per_tok", 0) or 0) if mc.num_experts else 0
         mc.weight_format = int(weight_format)
         self.weight_format = int(weight_format)
+        mc.kv_cache_dtype = int(kv_cache_dtype)
+        self.kv_cache_dtype = int(kv_cache_dtype)
         self.device = device
         self.tp_size, self.tp_rank = tp_size, tp_rank
         # rope tables first: an unsupported rope_scaling type must fail before any device memory is taken

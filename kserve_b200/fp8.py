@@ -13,6 +13,10 @@ loaded with W' (`dequantize_reference`).
 FP8 engines run on one GPU (tensor parallelism is refused).  Activations stay bf16: a checkpoint with dynamic per-token
 FP8 input activations ("FP8-dynamic") is served as W8A16 and its outputs are not those of a runtime that quantizes
 activations.  Static activation scales are refused.
+
+FP8 KV cache (`--kv_cache_dtype fp8`, independent of the checkpoint's format): the KV pages hold float8_e4m3fn codes of
+k after RoPE and v, `quantize_kv` of the bf16 values a bf16 cache would hold (per-tensor scale 1, what vLLM does for a
+checkpoint without calibrated KV scales), and attention reads bf16(code), which is exact.
 """
 from __future__ import annotations
 
@@ -29,6 +33,30 @@ PROJECTIONS = ("self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj", "self
 
 class UnsupportedQuantization(ValueError):
     pass
+
+
+# --kv_cache_dtype names (vLLM's) -> b200_model_config_t.kv_cache_dtype
+KV_CACHE_DTYPES = {"auto": 0, "bfloat16": 0, "fp8": 1, "fp8_e4m3": 1}
+
+
+def kv_cache_format(name: str, tp_size: int = 1) -> int:
+    """--kv_cache_dtype -> 0 (bf16 KV pages) or 1 (float8_e4m3fn codes); raises UnsupportedQuantization"""
+    if name == "fp8_e5m2":
+        raise UnsupportedQuantization("--kv_cache_dtype fp8_e5m2 is not supported (the FP8 KV cache is float8_e4m3fn: "
+                                      "use fp8 or fp8_e4m3)")
+    if name not in KV_CACHE_DTYPES:
+        raise UnsupportedQuantization(f"--kv_cache_dtype {name!r} is not one of {sorted(KV_CACHE_DTYPES)}")
+    fmt = KV_CACHE_DTYPES[name]
+    if fmt == 1 and tp_size > 1:
+        raise UnsupportedQuantization(f"an FP8 KV cache with tensor parallelism (tensor_parallel_size={tp_size}) is not "
+                                      "supported")
+    return fmt
+
+
+def quantize_kv(x: torch.Tensor) -> torch.Tensor:
+    """The code an FP8 KV cache stores for each element of x: e4m3(clamp(x, -448, 448)), round to nearest even (NaN stays
+    NaN; torch's plain cast would turn |x| >= 464 into NaN)"""
+    return x.float().clamp(-448.0, 448.0).to(torch.float8_e4m3fn)
 
 
 def _refuse(msg: str):

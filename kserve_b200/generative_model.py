@@ -22,7 +22,7 @@ import numpy as np
 import torch
 
 from .engine import B200Engine, GenerateResult
-from .fp8 import UnsupportedQuantization, log_activation_scheme, parse_quantization_config
+from .fp8 import UnsupportedQuantization, kv_cache_format, log_activation_scheme, parse_quantization_config
 from .utils import get_and_verify_max_len, logger, plan_memory, rope_inv_freq
 from .kserve_api.errors import InvalidInput
 from .kserve_api.metrics import DECODE_TOKENS_PER_S, LLM_STATS_KEY, TTFT_HIST, LLMStats, get_labels
@@ -118,7 +118,8 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
                  tokenizer=None, pad_token_id: Optional[int] = None, max_model_len: Optional[int] = None,
                  max_batch: int = 32, device: int = 0, tensor_parallel_size: int = 1, tp_rank: int = 0,
                  nccl_id: Optional[bytes] = None, system_fingerprint: Optional[str] = None,
-                 request_logger=None, continuous_batching: bool = False, generation_defaults: Optional[dict] = None):
+                 request_logger=None, continuous_batching: bool = False, generation_defaults: Optional[dict] = None,
+                 kv_cache_dtype: str = "auto"):
         Model.__init__(self, model_name)
         self.ready = False
         self.model_id_or_path = model_id_or_path
@@ -131,6 +132,7 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
         self.max_batch = max_batch
         self.device_index = device
         self.tp_size, self.tp_rank, self.nccl_id = tensor_parallel_size, tp_rank, nccl_id
+        self.kv_cache_dtype = kv_cache_dtype      # "auto" / "bfloat16" = bf16 KV pages; "fp8" / "fp8_e4m3" = e4m3 codes
         self.system_fingerprint = system_fingerprint
         self.request_logger = request_logger
         self.is_encoder_decoder = False
@@ -202,6 +204,10 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
             raise OpenAIError(str(e))
         if quant is not None:
             log_activation_scheme(quant)
+        try:
+            kv_format = kv_cache_format(self.kv_cache_dtype, self.tp_size)
+        except UnsupportedQuantization as e:
+            raise OpenAIError(str(e))
         # checkpoint generation defaults: transformers merges the None fields of the request's GenerationConfig from
         # model.generation_config (generation/utils.py:1693-1701) — this is how instruct checkpoints turn sampling on (q9)
         self.generation_defaults = dict(self._generation_defaults or {})
@@ -220,7 +226,7 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
         try:
             if torch.cuda.is_available():
                 cap_t, pages = plan_memory(cfg, vocab_rows, self.max_batch, self.max_length, self.tp_size,
-                                           torch.cuda.mem_get_info(self.device_index)[0])
+                                           torch.cuda.mem_get_info(self.device_index)[0], kv_bytes=1 if kv_format else 2)
             else:       # B200Engine raises below (no CPU fallback); nothing to plan
                 cap_t, pages = None, self.max_batch * -(-self.max_length // 64)
         except ValueError as e:
@@ -232,7 +238,7 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
         self._engine = B200Engine(cfg, max_batch=self.max_batch, max_seq_len=self.max_length, device=self.device_index,
                                   max_prefill_tokens=cap_t, num_kv_pages=pages,
                                   tp_rank=self.tp_rank, tp_size=self.tp_size, nccl_id=self.nccl_id, vocab_rows=vocab_rows,
-                                  weight_format=0 if quant is None else 1)
+                                  weight_format=0 if quant is None else 1, kv_cache_dtype=kv_format)
         weights = self._state_dict if self._state_dict is not None else load_safetensors_dir(self.model_id_or_path)
         V0 = cfg["vocab_size"]
 

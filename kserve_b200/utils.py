@@ -141,14 +141,15 @@ def hf_rope_tables(cfg: Dict[str, Any], head_dim: int, max_pos: int) -> Tuple[to
 
 
 def plan_memory(cfg: Dict[str, Any], vocab_rows: int, max_batch: int, max_len: int, tp_size: int, free_bytes: int,
-                max_prefill_tokens: Optional[int] = None, reserve_bytes: int = 3 << 30) -> Tuple[int, int]:
+                max_prefill_tokens: Optional[int] = None, reserve_bytes: int = 3 << 30, kv_bytes: int = 2) -> Tuple[int, int]:
     """-> (max_prefill_tokens, num_kv_pages) that fit `free_bytes` of device memory next to the weights.
 
     The engine preallocates its activation buffers for `max_prefill_tokens` packed prompt tokens and a pool of 64-token
     KV pages; sizing both as max_batch x max_model_len (a Llama-3.1 config says 131072) would not fit any GPU, so the
     prefill buffers are capped (one full-length prompt always fits) and the page pool takes what is left, at most
     max_batch full-length sequences and at least one.  An FP8 checkpoint (kserve_b200/fp8.py) keeps one byte per
-    projection weight plus a bf16 scale per row, and a bf16 scratch of one layer's projections for prefill."""
+    projection weight plus a bf16 scale per row, and a bf16 scratch of one layer's projections for prefill.  kv_bytes:
+    bytes per KV element, 2 for the bf16 cache, 1 for the FP8 one (twice the pages for the same memory)."""
     H, I, L = cfg["hidden_size"], cfg["intermediate_size"], cfg["num_hidden_layers"]
     nh, nkv = cfg["num_attention_heads"], cfg["num_key_value_heads"]
     d = cfg.get("head_dim") or H // nh
@@ -163,7 +164,7 @@ def plan_memory(cfg: Dict[str, Any], vocab_rows: int, max_batch: int, max_len: i
         weights -= L * (2 * linear - (linear + 2 * scale_rows))
         weights += 2 * linear
     per_tok = 2 * (3 * H + qkv_cols + nh_l * d + I_l) + 16 + (2 * (3 * H + 2 * I_l) + 24 if E else 0)
-    page = L * 2 * nkv_l * 64 * d * 2
+    page = L * 2 * nkv_l * 64 * d * kv_bytes
     pages_per_seq = -(-max_len // 64)
     want_pages = max_batch * pages_per_seq
     fixed = reserve_bytes + 3 * 8 * max_batch * max_len + 2 * 4 * max_batch * max_len + 2 * max_batch * -(-vocab_rows // tp_size)

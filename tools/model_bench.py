@@ -3,6 +3,7 @@
     python tools/model_bench.py                       # Qwen2.5-7B dims (28 layers), batch 32, 1024-in / 128-out
     python tools/model_bench.py --model llama3_8b --steps 3
     python tools/model_bench.py --model llama3_8b --weights fp8       # FP8 projections (e4m3 + a bf16 scale per row)
+    python tools/model_bench.py --model llama3_8b --kv-cache fp8      # FP8 KV cache (one e4m3 code per K / V element)
 
 The prompt is staged on the device once; each timed step is one prefill + (gen_len - 1) decode steps, measured with CUDA
 events on the engine stream (b200_run_staged_timed).  Prints one JSON line: output tok/s, TTFT, decode ms/step, and the
@@ -23,12 +24,12 @@ HBM_BYTES_PER_S = 3.35e12     # H100 SXM data sheet
 BF16_FLOPS = 989e12           # H100 SXM data sheet, dense
 
 
-def algorithmic(cfg, B, S, T, fp8=False):
+def algorithmic(cfg, B, S, T, fp8=False, kv8=False):
     H, I, V, L = cfg["hidden_size"], cfg["intermediate_size"], cfg["vocab_size"], cfg["num_hidden_layers"]
     nh, nkv, d = cfg["num_attention_heads"], cfg["num_key_value_heads"], cfg.get("head_dim") or H // cfg["num_attention_heads"]
     layer = (nh + 2 * nkv) * d * H + H * nh * d + 3 * H * I       # q/k/v, o, gate/up/down weights
     gemm_params = L * layer + V * H                                # + LM head (the embedding is a gather)
-    kv_per_token = 2 * L * nkv * d * 2                            # k and v, bf16
+    kv_per_token = 2 * L * nkv * d * (1 if kv8 else 2)           # k and v, bf16 or e4m3 codes
     mean_ctx = S + T / 2
     # FP8: one byte per projection weight plus a bf16 scale per row; the LM head stays bf16
     weight_bytes = (L * (layer + 2 * ((nh + 2 * nkv) * d + 2 * H + 2 * I)) + 2 * V * H) if fp8 else 2 * gemm_params
@@ -85,18 +86,21 @@ def main():
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--weights", choices=("bf16", "fp8"), default="bf16")
+    ap.add_argument("--kv-cache", choices=("bf16", "fp8"), default="bf16")
     args = ap.parse_args()
     from tools.synth_weights import CONFIGS
     cfg = CONFIGS[args.model]
     B, S, T = args.batch, args.prompt_len, args.gen_len
     fp8 = args.weights == "fp8"
-    alg = algorithmic(cfg, B, S, T, fp8)
+    kv8 = args.kv_cache == "fp8"
+    alg = algorithmic(cfg, B, S, T, fp8, kv8)
 
     import torch
     from kserve_b200.engine import B200Engine
     if not torch.cuda.is_available():
         raise SystemExit("model_bench needs a CUDA device: there is no CPU path to time")
-    eng = B200Engine(cfg, max_batch=B, max_seq_len=S + T, max_prefill_tokens=B * S, weight_format=1 if fp8 else 0)
+    eng = B200Engine(cfg, max_batch=B, max_seq_len=S + T, max_prefill_tokens=B * S, weight_format=1 if fp8 else 0,
+                     kv_cache_dtype=1 if kv8 else 0)
     eng.load_weights(device_weights(cfg, torch.device("cuda", 0), fp8))
     torch.cuda.empty_cache()
     g = torch.Generator().manual_seed(1234)
@@ -115,7 +119,7 @@ def main():
     ttft = statistics.median(pre)
     dec_step = statistics.median(dec) / (T - 1)
     line = dict(
-        model=args.model, weights=args.weights, batch=B, prompt_len=S, gen_len=T, steps=args.steps, warmup=args.warmup,
+        model=args.model, weights=args.weights, kv_cache=args.kv_cache, batch=B, prompt_len=S, gen_len=T, steps=args.steps, warmup=args.warmup,
         tok_per_s=round(B * T / (step_ms / 1e3), 1), ttft_ms=round(ttft, 1), decode_ms_per_step=round(dec_step, 3),
         ttft_ms_all=[round(x, 1) for x in pre], decode_ms_per_step_all=[round(x / (T - 1), 3) for x in dec],
         decode_bytes_per_step=alg["decode_bytes_per_step"], weight_bytes=alg["weight_bytes"],
