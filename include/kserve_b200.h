@@ -250,6 +250,23 @@ int b200_op_rope_kv(const void* qkv, int64_t ld, void* q_out, int64_t ldq, void*
                     const int32_t* page_table, int max_pages, const int32_t* tok_seq, const int32_t* tok_pos,
                     const void* cos_tab, const void* sin_tab, int T, int nh, int nkv, void* stream);
 int b200_op_argmax(const void* logits, int64_t ld, int B, int V, float* out_val, int32_t* out_idx, void* stream);
+/* The sparse MoE block of one layer, launched exactly as the engine launches it (Mixtral, top-2 routing).
+ * mode: 0 prefill (row-major expert GEMMs bounded by the device-side counts), 1 decode with one grouped swap-AB launch
+ * per projection (T <= 64), 2 decode with one launch per expert and the down projection cut into `splits` >= 1 K slices
+ * (splits > 1: fp32 partials in `part` [E][splits][T][H], summed by the combine; T <= 64).
+ * Weights (bf16): wr [E][H]; wgu [E][2I][H], expert e's gate rows g and up rows u interleaved in groups of 16 rows
+ * (rows 32j .. 32j+15 = g[16j ..], rows 32j+16 .. 32j+31 = u[16j ..]); wdown [E][H][I]; norm_w [H] (the next RMSNorm).
+ * In: xn [T][H] (routed and expert input), x [T][H] (residual).  Out, all on the device:
+ *   tok_expert int32 [T][2] (top-2, the lowest index wins ties), tok_weight fp32 [T][2] (renormalised),
+ *   count int32 [E], off int32 [E + 1] (exclusive scan of count rounded up to 8 rows; off[E] = total),
+ *   tok_row int32 [T][2] (row of each (token, k) in its expert's segment, token order within a segment),
+ *   xg [g_rows][H], hg [g_rows][I], yg [g_rows][H] (bf16, rows of the segments only; g_rows >= 2T + 8E),
+ *   then x <- bf16(x + combine), xn <- RMSNorm(x) * norm_w, or, when ysum [T][H] is non-NULL, ysum <- combine and
+ *   x / xn unchanged. */
+int b200_op_moe_block(int mode, const void* wr, const void* wgu, const void* wdown, const void* norm_w, void* x, void* xn,
+                      int T, int H, int I, int E, float eps, int32_t* tok_expert, float* tok_weight, int32_t* count,
+                      int32_t* off, int32_t* tok_row, void* xg, void* hg, void* yg, int g_rows, float* part, int splits,
+                      void* ysum, void* stream);
 
 /* Host-DRAM KV tier (BASELINE.json configs[3]): move all KV pages of staged sequence `slot` to pinned host memory /
  * back to the device, asynchronously on the engine stream.  scrub != 0 overwrites the device pages after the copy

@@ -297,6 +297,87 @@ static int allreduce_bf16(b200_engine* e, bf16* buf, size_t count, cudaStream_t 
   return 0;
 }
 
+// ---- sparse MoE block of one layer (route, group rows per expert, expert GEMMs bounded by the device-side counts,
+// combine + residual + next RMSNorm).  forward_layers and b200_op_moe_block both launch it through here.
+enum MoeMode : int { MOE_PREFILL = 0, MOE_DECODE_GROUPED = 1, MOE_DECODE_PER_EXPERT = 2 };
+
+struct MoeBlock {
+  int T, H, I, E;            // T token rows (decode: T == batch)
+  float eps;
+  const bf16* wr;            // router [E][H]
+  const bf16* wgu;           // [E][2I][H], every expert's gate / up rows in the 16-row interleave (EPI_SWIGLU)
+  const bf16* wdown;         // [E][H][I]
+  const bf16* next_norm;     // [H]
+  bf16* x; bf16* xn;         // [T][H]: residual stream (updated in place) and its next RMSNorm (input: this norm)
+  int32_t* tok_expert; float* tok_weight; int32_t* tok_row;   // [T][2]
+  int32_t* count; int32_t* off;                               // [E], [E + 1]
+  bf16* xg; bf16* hg; bf16* yg; int g_rows;                   // [g_rows][H], [g_rows][I], [g_rows][H]
+  float* part; int splits;   // per-expert decode, splits > 1: down-projection partials [E][splits][T][H]
+  bf16* ysum;                // non-null: the combined expert outputs go here, x / xn are left to the caller (TP)
+  float* sk_ws; int* sk_flags; int sk_tiles; size_t sk_ws_floats;   // stream-K workspace of the per-expert gate/up
+};
+
+static int launch_moe_block(TmapCache& tmaps, const MoeBlock& m, int mode, int sms, cudaStream_t s, int* launches) {
+  const int T = m.T, H = m.H, I = m.I, E = m.E;
+  const bool decode = mode != MOE_PREFILL;
+  const int bn = pick_block_n(T);
+  int rc;
+  if (decode && T <= kMoeDecodeMaxT) {
+    B200_CUDA_OK(launch_k(moe_router_decode_kernel, dim3(T), dim3(32 * E), 0, s, (const bf16*)m.xn, m.wr, H, E, m.tok_expert, m.tok_weight));
+    B200_CUDA_OK(launch_k(moe_place_gather_kernel, dim3(T), dim3(256), 0, s, (const bf16*)m.xn, (const int32_t*)m.tok_expert, T, H, E,
+                          m.count, m.off, m.tok_row, m.xg));
+    *launches += 2;
+  } else {
+    B200_CUDA_OK(launch_k(moe_router_kernel, dim3((T + 3) / 4), dim3(128), 0, s, (const bf16*)m.xn, m.wr, T, H, E, m.tok_expert, m.tok_weight));
+    B200_CUDA_OK(launch_k(moe_offsets_kernel, dim3(1), dim3(1024), 0, s, (const int32_t*)m.tok_expert, T, E, m.count, m.off, m.tok_row));
+    B200_CUDA_OK(launch_k(moe_gather_kernel, dim3(T), dim3(128), 0, s, (const bf16*)m.xn, (const int32_t*)m.tok_row, m.xg, H));
+    *launches += 3;
+  }
+  // decode: ONE grouped launch per projection over all experts (E * tiles fill the SMs; the weights of experts
+  // without tokens are skipped), or one launch per expert with the down projection split over K
+  const int dsp = mode == MOE_DECODE_PER_EXPERT ? m.splits : 1;
+  if (mode == MOE_DECODE_GROUPED) {
+    GemmArgs a{m.wgu, E * 2 * I, m.xg, m.g_rows, 2 * I, T, H, EPI_T_SWIGLU, bn, 1, m.hg, nullptr, I, 0, I, true};
+    a.n_rt = m.count; a.row_off = m.off; a.groups = E;
+    if ((rc = launch_gemm(tmaps, a, sms, s))) return rc;
+    GemmArgs d{m.wdown, E * H, m.hg, m.g_rows, H, T, I, EPI_T_STORE, bn, 1, m.yg, nullptr, H, 0, 0, true};
+    d.n_rt = m.count; d.row_off = m.off; d.groups = E;
+    if ((rc = launch_gemm(tmaps, d, sms, s))) return rc;
+    *launches += 2;
+  }
+  for (int x = 0; x < E && mode != MOE_DECODE_GROUPED; ++x) {
+    const bf16* wgu = m.wgu + (long long)x * 2 * I * H;
+    const bf16* wdn = m.wdown + (long long)x * H * I;
+    if (decode) {
+      GemmArgs a{wgu, 2 * I, m.xg, m.g_rows, 2 * I, T, H, EPI_T_SWIGLU, bn, 1, m.hg, nullptr, I, 0, I, true};
+      a.sk_ws = m.sk_ws; a.sk_flags = m.sk_flags; a.sk_tiles = m.sk_tiles; a.sk_ws_floats = m.sk_ws_floats;
+      a.n_rt = m.count + x; a.row_off = m.off + x;
+      if ((rc = launch_gemm(tmaps, a, sms, s))) return rc;
+      GemmArgs d{wdn, H, m.hg, m.g_rows, H, T, I, dsp > 1 ? EPI_T_PARTIAL : EPI_T_STORE, bn, dsp,
+                 dsp > 1 ? (void*)(m.part + (size_t)x * dsp * T * H) : (void*)m.yg, nullptr, H, (long long)T * H, 0, true};
+      d.n_rt = m.count + x; d.row_off = m.off + x;
+      if ((rc = launch_gemm(tmaps, d, sms, s))) return rc;
+    } else {
+      GemmArgs a{m.xg, m.g_rows, wgu, 2 * I, T, 2 * I, H, EPI_SWIGLU, 256, 1, m.hg, nullptr, I, 0, I, false};
+      a.m_rt = m.count + x; a.row_off = m.off + x;
+      if ((rc = launch_gemm(tmaps, a, sms, s))) return rc;
+      GemmArgs d{m.hg, m.g_rows, wdn, H, T, H, I, EPI_STORE, 256, 1, m.yg, nullptr, H, 0, 0, false};
+      d.m_rt = m.count + x; d.row_off = m.off + x;
+      if ((rc = launch_gemm(tmaps, d, sms, s))) return rc;
+    }
+    *launches += 2;
+  }
+  MoeCombineParams cp{};
+  cp.x = m.x; cp.w = m.next_norm; cp.xn = m.xn; cp.H = H; cp.eps = m.eps;
+  cp.tok_expert = m.tok_expert; cp.tok_weight = m.tok_weight; cp.tok_row = m.tok_row; cp.off = m.off;
+  cp.yg = m.yg;
+  if (dsp > 1) { cp.part = m.part; cp.splits = dsp; cp.expert_stride = (long long)dsp * T * H; cp.split_stride = (long long)T * H; }
+  cp.ysum = m.ysum;
+  B200_CUDA_OK(launch_k(moe_combine_norm_kernel, dim3(T), dim3(kNormThreads), (size_t)(H + 32) * sizeof(float), s, cp));
+  *launches += 1;
+  return 0;
+}
+
 // ---- one transformer stack pass over T token rows --------------------------------------------------
 // decode == true : T == B rows, swap-AB GEMMs (+ split-K), flash-decoding attention
 // decode == false: packed prompt tokens, row-major GEMMs, causal flash attention
@@ -513,64 +594,15 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
     if ((rc = row_parallel(e->attn, e->nh * kHeadDim, w.wo, w.wo8, w.so, w.ln2))) return rc;
     const bf16* next_norm = (l + 1 < e->L) ? e->layers[l + 1].ln1 : e->final_norm;
     if (e->E > 0) {
-      // ---- sparse MoE: route, group rows per expert, run the expert GEMMs bounded by the device-side counts, combine
-      if (decode && T <= kMoeDecodeMaxT) {
-        B200_CUDA_OK(launch_k(moe_router_decode_kernel, dim3(T), dim3(32 * e->E), 0, s, (const bf16*)e->xn, (const bf16*)w.wr, H, e->E,
-                              e->tok_expert, e->tok_weight));
-        B200_CUDA_OK(launch_k(moe_place_gather_kernel, dim3(T), dim3(256), 0, s, (const bf16*)e->xn, (const int32_t*)e->tok_expert, T, H, e->E,
-                              e->e_count, e->e_off, e->tok_row, e->xg));
-        e->launches += 2;
-      } else {
-        B200_CUDA_OK(launch_k(moe_router_kernel, dim3((T + 3) / 4), dim3(128), 0, s, (const bf16*)e->xn, (const bf16*)w.wr, T, H, e->E,
-                              e->tok_expert, e->tok_weight));
-        B200_CUDA_OK(launch_k(moe_offsets_kernel, dim3(1), dim3(1024), 0, s, (const int32_t*)e->tok_expert, T, e->E, e->e_count, e->e_off, e->tok_row));
-        B200_CUDA_OK(launch_k(moe_gather_kernel, dim3(T), dim3(128), 0, s, (const bf16*)e->xn, (const int32_t*)e->tok_row, e->xg, H));
-        e->launches += 3;
-      }
-      // decode: ONE grouped launch per projection over all experts (E * tiles fill the SMs; the weights of experts
-      // without tokens are skipped).  B200_MOE_PER_EXPERT=1 restores one launch per expert (A/B).
+      // B200_MOE_PER_EXPERT=1: one launch per expert instead of the grouped decode launches (A/B)
       static const bool per_expert = getenv("B200_MOE_PER_EXPERT") != nullptr;
-      const bool grouped = decode && !per_expert;
-      const int dsp = (decode && !grouped) ? pick_splits(e, H, e->I) : 1;
-      if (grouped) {
-        GemmArgs a{w.wgu_e, e->E * 2 * e->I, e->xg, e->g_rows, 2 * e->I, B, H, EPI_T_SWIGLU, bn, 1, e->hg, nullptr, e->I, 0, e->I, true};
-        a.n_rt = e->e_count; a.row_off = e->e_off; a.groups = e->E;
-        if ((rc = launch_gemm(e, a, e->num_sms, s))) return rc;
-        GemmArgs d{w.wdown_e, e->E * H, e->hg, e->g_rows, H, B, e->I, EPI_T_STORE, bn, 1, e->yg, nullptr, H, 0, 0, true};
-        d.n_rt = e->e_count; d.row_off = e->e_off; d.groups = e->E;
-        if ((rc = launch_gemm(e, d, e->num_sms, s))) return rc;
-        e->launches += 2;
-      }
-      for (int x = 0; x < e->E && !grouped; ++x) {
-        const bf16* wgu = w.wgu_e + (long long)x * 2 * e->I * H;
-        const bf16* wdn = w.wdown_e + (long long)x * H * e->I;
-        if (decode) {
-          GemmArgs a{wgu, 2 * e->I, e->xg, e->g_rows, 2 * e->I, B, H, EPI_T_SWIGLU, bn, 1, e->hg, nullptr, e->I, 0, e->I, true};
-          a.sk_ws = e->sk_ws; a.sk_flags = e->sk_flags; a.sk_tiles = e->sk_tiles; a.sk_ws_floats = e->sk_ws_floats;
-          a.n_rt = e->e_count + x; a.row_off = e->e_off + x;
-          if ((rc = launch_gemm(e, a, e->num_sms, s))) return rc;
-          GemmArgs d{wdn, H, e->hg, e->g_rows, H, B, e->I, dsp > 1 ? EPI_T_PARTIAL : EPI_T_STORE, bn, dsp,
-                     dsp > 1 ? (void*)(e->ws + (size_t)x * dsp * B * H) : (void*)e->yg, nullptr, H, (long long)B * H, 0, true};
-          d.n_rt = e->e_count + x; d.row_off = e->e_off + x;
-          if ((rc = launch_gemm(e, d, e->num_sms, s))) return rc;
-        } else {
-          GemmArgs a{e->xg, e->g_rows, wgu, 2 * e->I, T, 2 * e->I, H, EPI_SWIGLU, 256, 1, e->hg, nullptr, e->I, 0, e->I, false};
-          a.m_rt = e->e_count + x; a.row_off = e->e_off + x;
-          if ((rc = launch_gemm(e, a, gsms, s))) return rc;
-          GemmArgs d{e->hg, e->g_rows, wdn, H, T, H, e->I, EPI_STORE, 256, 1, e->yg, nullptr, H, 0, 0, false};
-          d.m_rt = e->e_count + x; d.row_off = e->e_off + x;
-          if ((rc = launch_gemm(e, d, gsms, s))) return rc;
-        }
-        e->launches += 2;
-      }
-      MoeCombineParams cp{};
-      cp.x = e->x; cp.w = next_norm; cp.xn = e->xn; cp.H = H; cp.eps = eps;
-      cp.tok_expert = e->tok_expert; cp.tok_weight = e->tok_weight; cp.tok_row = e->tok_row; cp.off = e->e_off;
-      cp.yg = e->yg;
-      if (decode && dsp > 1) { cp.part = e->ws; cp.splits = dsp; cp.expert_stride = (long long)dsp * B * H; cp.split_stride = (long long)B * H; }
-      cp.ysum = tp ? e->ybuf : nullptr;
-      B200_CUDA_OK(launch_k(moe_combine_norm_kernel, dim3(T), dim3(kNormThreads), (size_t)(H + 32) * sizeof(float), s, cp));
-      e->launches++;
+      const int mode = !decode ? MOE_PREFILL : (per_expert ? MOE_DECODE_PER_EXPERT : MOE_DECODE_GROUPED);
+      MoeBlock mb{T, H, e->I, e->E, eps, w.wr, w.wgu_e, w.wdown_e, next_norm, e->x, e->xn,
+                  e->tok_expert, e->tok_weight, e->tok_row, e->e_count, e->e_off, e->xg, e->hg, e->yg, e->g_rows,
+                  e->ws, mode == MOE_DECODE_PER_EXPERT ? pick_splits(e, H, e->I) : 1, tp ? e->ybuf : nullptr,
+                  e->sk_ws, e->sk_flags, e->sk_tiles, e->sk_ws_floats};
+      // (the MoE GEMMs have device-side extents, so none of them is pf_eligible: launch_gemm(e, ...) would add nothing)
+      if ((rc = launch_moe_block(e->tmaps, mb, mode, decode ? e->num_sms : gsms, s, &e->launches))) return rc;
       if (tp && decode && e->p2p_ready) {   // all-reduce of the combined expert outputs + residual + next norm, over peer memory
         B200_CUDA_OK(launch_k(ar_kernel(e), dim3(T), dim3(kNormThreads), (size_t)(H + 32) * sizeof(float), s, e->p2p,
                               e->x, next_norm, e->xn, eps, (const float*)nullptr, 0, 0LL, 0LL, (const bf16*)e->ybuf,
@@ -2466,6 +2498,34 @@ int b200_op_argmax(const void* logits, int64_t ld, int B, int V, float* out_val,
   argmax_kernel<<<dim3(B, 1), 1024, 0, (cudaStream_t)stream>>>((const bf16*)logits, ld, V, 0, out_val, out_idx, P2P{}, 0);
   B200_CUDA_OK(cudaGetLastError());
   return 0;
+}
+
+int b200_op_moe_block(int mode, const void* wr, const void* wgu, const void* wdown, const void* norm_w, void* x, void* xn,
+                      int T, int H, int I, int E, float eps, int32_t* tok_expert, float* tok_weight, int32_t* count,
+                      int32_t* off, int32_t* tok_row, void* xg, void* hg, void* yg, int g_rows, float* part, int splits,
+                      void* ysum, void* stream) {
+  B200_REQUIRE(mode >= MOE_PREFILL && mode <= MOE_DECODE_PER_EXPERT, "b200_op_moe_block: mode 0, 1 or 2");
+  B200_REQUIRE(E >= 2 && E <= kMaxExperts && T >= 1 && H % 64 == 0 && I % 64 == 0, "b200_op_moe_block: 2..16 experts, H and I multiples of 64");
+  B200_REQUIRE(mode == MOE_PREFILL || T <= kMoeDecodeMaxT, "b200_op_moe_block: decode modes take at most 64 rows");
+  B200_REQUIRE(g_rows >= 2 * T + 8 * E, "b200_op_moe_block: g_rows must hold every expert segment (2T + 8E rows)");
+  const int sp = mode == MOE_DECODE_PER_EXPERT ? splits : 1;
+  B200_REQUIRE(sp >= 1 && effective_splits(I, sp) == sp && (sp == 1 || part != nullptr),
+               "b200_op_moe_block: splits >= 1 that split I without an empty slice, and `part` when splits > 1");
+  g_op_tmaps.maps.clear();  // caller buffers may be reused at other shapes
+  static float* sk_ws = nullptr;
+  static int* sk_flags = nullptr;
+  const int sk_tiles = 2048;
+  const size_t sk_floats = (size_t)sk_tiles * 2 * 64 * kGemmBlockM;
+  if (mode == MOE_DECODE_PER_EXPERT && !sk_ws) {
+    B200_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&sk_ws), sk_floats * sizeof(float)));
+    B200_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&sk_flags), sk_tiles * sizeof(int)));
+    B200_CUDA_OK(cudaMemset(sk_flags, 0, sk_tiles * sizeof(int)));
+  }
+  MoeBlock m{T, H, I, E, eps, (const bf16*)wr, (const bf16*)wgu, (const bf16*)wdown, (const bf16*)norm_w, (bf16*)x, (bf16*)xn,
+             tok_expert, tok_weight, tok_row, count, off, (bf16*)xg, (bf16*)hg, (bf16*)yg, g_rows, part, sp, (bf16*)ysum,
+             sk_ws, sk_flags, sk_tiles, sk_floats};
+  int launches = 0;
+  return launch_moe_block(g_op_tmaps, m, mode, op_sms(), (cudaStream_t)stream, &launches);
 }
 
 }  // extern "C"
