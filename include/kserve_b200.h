@@ -250,6 +250,16 @@ int b200_op_rope_kv(const void* qkv, int64_t ld, void* q_out, int64_t ldq, void*
                     const int32_t* page_table, int max_pages, const int32_t* tok_seq, const int32_t* tok_pos,
                     const void* cos_tab, const void* sin_tab, int T, int nh, int nkv, void* stream);
 int b200_op_argmax(const void* logits, int64_t ld, int B, int V, float* out_val, int32_t* out_idx, void* stream);
+/* The logits processors and the draw of one decode step, launched exactly as the engine launches them (one CTA of 1024
+ * threads per row).  logits bf16 [B][ld] (ld >= V); params are mapped as b200_generate / b200_cb_admit map them.
+ *   row_slot NULL (static batch): params[0] for every row, seen row b = batch row b, RNG counter (step, b)
+ *   row_slot int32 [B] (continuous batching): row b uses slot row_slot[b]: params[slot], seen row slot, RNG counter
+ *            (n_gen[slot], 0); n_cfg = number of slots
+ * seen: uint32 [rows][(V + 31) / 32] token-presence bitmaps for the repetition penalty, or NULL.
+ * Out (device): out_idx int32 [B] the selected token, out_val fp32 [B] its processed score. */
+int b200_op_sample(const void* logits, int64_t ld, int B, int V, const uint32_t* seen, const int32_t* row_slot,
+                   const int32_t* n_gen, int n_cfg, const b200_gen_params_t* params, int32_t step, float* out_val,
+                   int32_t* out_idx, void* stream);
 /* The sparse MoE block of one layer, launched exactly as the engine launches it (Mixtral, top-2 routing).
  * mode: 0 prefill (row-major expert GEMMs bounded by the device-side counts), 1 decode with one grouped swap-AB launch
  * per projection (T <= 64), 2 decode with one launch per expert and the down projection cut into `splits` >= 1 K slices

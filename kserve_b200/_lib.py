@@ -85,6 +85,7 @@ def load() -> C.CDLL:
     lib.b200_op_rope_kv.argtypes = [vp, i64, vp, i64, vp, vp, vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int,
                                     C.c_int, vp]
     lib.b200_op_argmax.argtypes = [vp, i64, C.c_int, C.c_int, vp, vp, vp]
+    lib.b200_op_sample.argtypes = [vp, i64, C.c_int, C.c_int, vp, vp, vp, C.c_int, C.POINTER(GenParams), i32, vp, vp, vp]
     lib.b200_op_moe_block.argtypes = [C.c_int, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                       vp, vp, vp, vp, vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp]
     lib.b200_batch_predict.argtypes = [vp, vp, vp, i32, C.POINTER(GenParams), vp, C.POINTER(i32), C.POINTER(i32)]

@@ -781,6 +781,21 @@ static int decode_step(b200_engine* e, bool use_graph) {
   return graph_step(e, key, [&] { return decode_step_enqueue(e); });
 }
 
+// b200_gen_params_t -> the kernel's configuration: 0 selects each field's default, top_k is capped at kSampleMaxCand.
+// NULL gives greedy decoding without processors.  Static batches, continuous batching and b200_op_sample all map here.
+static SampleCfg sample_cfg(const b200_gen_params_t* gp) {
+  SampleCfg sc{};
+  sc.rep_penalty = 1.0f; sc.temperature = 1.0f; sc.top_p = 1.0f; sc.top_k = 50;
+  if (!gp) return sc;
+  sc.rep_penalty = (gp->repetition_penalty > 0.f) ? gp->repetition_penalty : 1.0f;
+  sc.temperature = (gp->temperature > 0.f) ? gp->temperature : 1.0f;
+  sc.do_sample = gp->do_sample ? 1 : 0;
+  sc.top_p = (gp->top_p > 0.f && gp->top_p < 1.f) ? gp->top_p : 1.0f;
+  sc.top_k = gp->top_k > 0 ? std::min(gp->top_k, kSampleMaxCand) : 50;
+  sc.seed = gp->seed;
+  return sc;
+}
+
 // Validates the request, sizes the KV pages and resets the per-request device state.  `lens` are the real
 // (un-padded) sequence lengths; S is the padded prompt width (0 for ragged batcher input).
 static int stage_common(b200_engine* e, int B, int S, const std::vector<int>& lens, const b200_gen_params_t* gp) {
@@ -839,13 +854,7 @@ static int stage_common(b200_engine* e, int B, int S, const std::vector<int>& le
   *e->h_state = init;
   B200_CUDA_OK(cudaMemcpyAsync(e->d_state, e->h_state, sizeof(StepState), cudaMemcpyHostToDevice, s));
   // logits processors / sampling (build_generation_config, generative_model.py:388-402)
-  SampleCfg sc{};
-  sc.rep_penalty = (gp->repetition_penalty > 0.f) ? gp->repetition_penalty : 1.0f;
-  sc.temperature = (gp->temperature > 0.f) ? gp->temperature : 1.0f;
-  sc.do_sample = gp->do_sample ? 1 : 0;
-  sc.top_p = (gp->top_p > 0.f && gp->top_p < 1.f) ? gp->top_p : 1.0f;
-  sc.top_k = gp->top_k > 0 ? std::min(gp->top_k, kSampleMaxCand) : 50;
-  sc.seed = gp->seed;
+  const SampleCfg sc = sample_cfg(gp);
   st.rep_on = sc.rep_penalty != 1.0f;
   st.sample_on = st.rep_on || sc.do_sample;
   if (st.sample_on) {
@@ -1233,19 +1242,8 @@ static int cb_admit(b200_engine* e, int n, const int64_t* const* rows, const int
   B200_CUDA_OK(cudaGetLastError());
   // ---- logits processors / sampling per sequence (build_generation_config, generative_model.py:388-402)
   for (int i = 0; i < n; ++i) {
-    SampleCfg sc{};
-    sc.rep_penalty = 1.0f; sc.temperature = 1.0f; sc.top_p = 1.0f; sc.top_k = 50;
-    bool on = false;
-    if (sampling) {
-      const b200_gen_params_t& gp = sampling[i];
-      sc.rep_penalty = (gp.repetition_penalty > 0.f) ? gp.repetition_penalty : 1.0f;
-      sc.temperature = (gp.temperature > 0.f) ? gp.temperature : 1.0f;
-      sc.do_sample = gp.do_sample ? 1 : 0;
-      sc.top_p = (gp.top_p > 0.f && gp.top_p < 1.f) ? gp.top_p : 1.0f;
-      sc.top_k = gp.top_k > 0 ? std::min(gp.top_k, kSampleMaxCand) : 50;
-      sc.seed = gp.seed;
-      on = sc.rep_penalty != 1.0f || sc.do_sample;
-    }
+    const SampleCfg sc = sample_cfg(sampling ? sampling + i : nullptr);
+    const bool on = sc.rep_penalty != 1.0f || sc.do_sample;
     if (on && e->cfg.tp_size != 1) { rollback(n); set_last_error("logits processors / sampling run on one GPU per engine (tp_size == 1)"); return -2; }
     B200_CUDA_OK(cudaMemcpyAsync(e->d_cb_cfg + slots[i], &sc, sizeof(sc), cudaMemcpyHostToDevice, s));   // (pageable source: staged before return)
     if (on && sc.rep_penalty != 1.0f) {
@@ -2497,6 +2495,36 @@ int b200_op_rope_kv(const void* qkv, int64_t ld, void* q_out, int64_t ldq, void*
 int b200_op_argmax(const void* logits, int64_t ld, int B, int V, float* out_val, int32_t* out_idx, void* stream) {
   argmax_kernel<<<dim3(B, 1), 1024, 0, (cudaStream_t)stream>>>((const bf16*)logits, ld, V, 0, out_val, out_idx, P2P{}, 0);
   B200_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int b200_op_sample(const void* logits, int64_t ld, int B, int V, const uint32_t* seen, const int32_t* row_slot,
+                   const int32_t* n_gen, int n_cfg, const b200_gen_params_t* params, int32_t step, float* out_val,
+                   int32_t* out_idx, void* stream) {
+  B200_REQUIRE(B >= 1 && V >= 1 && ld >= V && params && out_val && out_idx, "b200_op_sample: B, V >= 1, ld >= V, params and outputs");
+  B200_REQUIRE(row_slot ? (n_gen != nullptr && n_cfg >= 1) : n_cfg == 1,
+               "b200_op_sample: one config without row_slot; with row_slot, n_gen and one config per slot");
+  cudaStream_t s = (cudaStream_t)stream;
+  static SampleCfg* d_cfg = nullptr;     // device copies of the configs and the step counter, kept across calls
+  static int cfg_cap = 0;
+  static StepState* d_st = nullptr;
+  if (n_cfg > cfg_cap) {
+    if (d_cfg) B200_CUDA_OK(cudaFree(d_cfg));
+    B200_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&d_cfg), (size_t)n_cfg * sizeof(SampleCfg)));
+    cfg_cap = n_cfg;
+  }
+  if (!d_st) B200_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&d_st), sizeof(StepState)));
+  std::vector<SampleCfg> cfg(n_cfg);
+  for (int i = 0; i < n_cfg; ++i) cfg[i] = sample_cfg(params + i);
+  const StepState st{step, 0, 0, 0};
+  B200_CUDA_OK(cudaMemcpyAsync(d_cfg, cfg.data(), cfg.size() * sizeof(SampleCfg), cudaMemcpyHostToDevice, s));   // (pageable: staged before return)
+  B200_CUDA_OK(cudaMemcpyAsync(d_st, &st, sizeof(st), cudaMemcpyHostToDevice, s));
+  SampleParams sp{};   // as head_and_step fills it
+  sp.logits = (const bf16*)logits; sp.ld = ld; sp.V = V; sp.words = (V + 31) / 32;
+  sp.seen = seen; sp.cfg = d_cfg; sp.out_val = out_val; sp.out_idx = out_idx;
+  if (row_slot) { sp.row_slot = row_slot; sp.n_gen = n_gen; }
+  else sp.st = d_st;
+  B200_CUDA_OK(launch_k(sample_kernel, dim3(B), dim3(1024), 0, s, sp));
   return 0;
 }
 

@@ -6,8 +6,10 @@
 //
 //   * repetition penalty: score = score > 0 ? score / p : score * p for every token id present in input_ids (prompt,
 //     pads included, + generated so far) — a bitmap [row][V/32] maintained by seen_init_kernel / step_update_kernel
-//   * top-k by an exact 4-pass radix select on the order-preserving uint32 image of the fp32 scores (ties with the
-//     k-th value are all kept, as `scores < topk[..., -1]` does), candidates sorted in shared memory
+//   * top-k by an exact 4-pass radix select on the order-preserving uint32 image of the fp32 scores; every tie with the
+//     k-th value is kept, as `scores < topk[..., -1]` does, however many there are (candidates above the k-th value and
+//     the ties that fit are sorted in shared memory; a draw among the rest counts the ties in index order)
+//   * top_k = 1 with do_sample draws among the tokens tied at the maximum; only do_sample = 0 is greedy
 //   * top-p exactly as TopPLogitsWarper: ascending cumulative probability <= 1 - top_p is removed, at least one kept
 //   * multinomial by inverse CDF with a Philox4x32-10 uniform keyed by (seed, step, row): reproducible per seed, but
 //     NOT torch's generator stream — sampled ids are distribution-equal, not bit-equal, to the reference
@@ -28,8 +30,9 @@ struct SampleCfg {             // device-resident (constant pointer inside CUDA 
 
 constexpr int kSampleMaxCand = 1024;
 
+// -0.0 maps to the key of +0.0: they compare equal, so top-k keeps both or neither
 __device__ __forceinline__ uint32_t f32_order_key(float f) {
-  const uint32_t u = __float_as_uint(f);
+  const uint32_t u = (f == 0.0f) ? 0u : __float_as_uint(f);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
@@ -78,7 +81,8 @@ struct SampleParams {
 };
 
 // one CTA of 1024 threads per row
-__global__ void __launch_bounds__(1024) sample_kernel(const SampleParams p) {
+// minimum 1 CTA per SM: ptxas otherwise plans two 1024-thread CTAs per SM, caps the kernel at 32 registers and spills
+__global__ void __launch_bounds__(1024, 1) sample_kernel(const SampleParams p) {
   TraceScope _ts(TK_ARGMAX);
   pdl_launch_dependents();
   pdl_wait();
@@ -87,7 +91,7 @@ __global__ void __launch_bounds__(1024) sample_kernel(const SampleParams p) {
   __shared__ float c_key[kSampleMaxCand];
   __shared__ int c_idx[kSampleMaxCand];
   __shared__ uint32_t s_prefix, s_remaining;
-  __shared__ int s_count;
+  __shared__ int s_count, s_ties, s_pick;
   __shared__ float sv[32];
   __shared__ int si[32];
   const int b = blockIdx.x, tid = threadIdx.x;
@@ -104,7 +108,7 @@ __global__ void __launch_bounds__(1024) sample_kernel(const SampleParams p) {
     if (sampling) x = x / temp;
     return x;
   };
-  if (!sampling || cfg.top_k <= 1) {
+  if (!sampling) {
     // ---- greedy over the processed scores (ties -> lowest index, like torch.argmax)
     float best = -INFINITY;
     int bi = 0x7fffffff;
@@ -135,7 +139,7 @@ __global__ void __launch_bounds__(1024) sample_kernel(const SampleParams p) {
   }
   // ---- top-k: radix select of the k-th largest order key
   const int k = min(min(cfg.top_k, kSampleMaxCand), p.V);
-  if (tid == 0) { s_prefix = 0; s_remaining = (uint32_t)k; s_count = 0; }
+  if (tid == 0) { s_prefix = 0; s_remaining = (uint32_t)k; s_count = 0; s_ties = 0; }
   for (int pass = 3; pass >= 0; --pass) {
     if (tid < 256) hist[tid] = 0;
     __syncthreads();
@@ -158,17 +162,26 @@ __global__ void __launch_bounds__(1024) sample_kernel(const SampleParams p) {
     }
     __syncthreads();
   }
+  // ---- kept set: the G = k - s_remaining tokens above the k-th key, then every tie at the k-th key (transformers keeps
+  // them all, `scores < kth` removes none of them).  Order: score descending, index ascending, so the ties come last and
+  // share one weight.  The G tokens go to c_[0, G); the ties follow from slot G while they fit.
   const uint32_t kth = s_prefix;
+  const int G = k - (int)s_remaining;
   for (int i = tid; i < p.V; i += blockDim.x) {
     const float x = score(i);
-    if (f32_order_key(x) >= kth) {
+    const uint32_t key = f32_order_key(x);
+    if (key > kth) {
       const int slot = atomicAdd(&s_count, 1);
+      c_key[slot] = x; c_idx[slot] = i;
+    } else if (key == kth) {
+      const int slot = G + atomicAdd(&s_ties, 1);
       if (slot < kSampleMaxCand) { c_key[slot] = x; c_idx[slot] = i; }
     }
   }
   __syncthreads();
-  const int n = min(s_count, kSampleMaxCand);
-  for (int i = n + tid; i < kSampleMaxCand; i += blockDim.x) { c_key[i] = -INFINITY; c_idx[i] = 0x7fffffff; }
+  const int n = G + s_ties;                    // kept tokens; candidate j >= G is a tie
+  const int nb = min(n, kSampleMaxCand);
+  for (int i = nb + tid; i < kSampleMaxCand; i += blockDim.x) { c_key[i] = -INFINITY; c_idx[i] = 0x7fffffff; }
   __syncthreads();
   // bitonic sort, descending by score, ascending index on ties
   for (int size = 2; size <= kSampleMaxCand; size <<= 1) {
@@ -185,22 +198,24 @@ __global__ void __launch_bounds__(1024) sample_kernel(const SampleParams p) {
     }
   }
   if (tid == 0) {
-    // softmax over the candidates, TopPLogitsWarper, renormalise, inverse-CDF draw
+    // softmax over the kept tokens, TopPLogitsWarper, renormalise, inverse-CDF draw
     const float m = c_key[0];
+    const float e_tie = expf(c_key[G] - m);
+    auto wt = [&](int j) { return j < G ? expf(c_key[j] - m) : e_tie; };
     float Z = 0.f;
-    for (int j = 0; j < n; ++j) Z += expf(c_key[j] - m);
+    for (int j = 0; j < n; ++j) Z += wt(j);
     int keep = n;
     if (cfg.top_p < 1.0f) {
       // ascending cumulative prob (tail sum from the smallest up to j) <= 1 - top_p  =>  removed
       float tail = 0.f;
       keep = 1;
       for (int j = n - 1; j >= 1; --j) {
-        tail += expf(c_key[j] - m) / Z;
+        tail += wt(j) / Z;
         if (tail > 1.0f - cfg.top_p) { keep = j + 1; break; }
       }
     }
     float Zk = 0.f;
-    for (int j = 0; j < keep; ++j) Zk += expf(c_key[j] - m);
+    for (int j = 0; j < keep; ++j) Zk += wt(j);
     const uint4 r = philox4x32_10(make_uint4(p.row_slot ? (uint32_t)p.n_gen[srow] : (uint32_t)p.st->step, p.row_slot ? 0u : (uint32_t)b, 0x5eed5eedu, 0u),
                                   make_uint2((uint32_t)cfg.seed, (uint32_t)(cfg.seed >> 32)));
     const float u = ((float)(r.x >> 8) + 0.5f) * (1.0f / 16777216.0f);   // (0, 1)
@@ -208,11 +223,30 @@ __global__ void __launch_bounds__(1024) sample_kernel(const SampleParams p) {
     float acc = 0.f;
     int pick = keep - 1;
     for (int j = 0; j < keep; ++j) {
-      acc += expf(c_key[j] - m);
+      acc += wt(j);
       if (acc >= target) { pick = j; break; }
     }
-    p.out_val[b] = c_key[pick];
-    p.out_idx[b] = c_idx[pick];
+    s_pick = pick;
+  }
+  __syncthreads();
+  const int pick = s_pick;
+  if (pick < G || n <= kSampleMaxCand) {       // the candidate buffer holds the pick
+    if (tid == 0) { p.out_val[b] = c_key[pick]; p.out_idx[b] = c_idx[pick]; }
+    return;
+  }
+  // more ties than the buffer holds: the pick is tie number pick - G in index order, found by an ordered block-wide count
+  const int want = pick - G, w = tid >> 5, l = tid & 31;
+  for (int t0 = 0, before = 0; t0 < p.V && before <= want; t0 += blockDim.x) {   // before: ties at indices < t0
+    const int i = t0 + tid;
+    const bool tie = i < p.V && f32_order_key(score(i)) == kth;
+    const uint32_t bal = __ballot_sync(0xffffffffu, tie);
+    if (l == 0) si[w] = __popc(bal);
+    __syncthreads();
+    int below = before + __popc(bal & ((1u << l) - 1u)), total = before;
+    for (int q = 0; q < 32; ++q) { total += si[q]; if (q < w) below += si[q]; }
+    if (tie && below == want) { p.out_val[b] = score(i); p.out_idx[b] = i; }
+    before = total;
+    __syncthreads();
   }
 }
 
