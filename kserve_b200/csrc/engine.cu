@@ -247,10 +247,11 @@ static ArKernel ar_kernel(const b200_engine* e) {
   return (e->cfg.tp_size >= min_tp && (e->H / e->cfg.tp_size) % 8 == 0) ? allreduce2_norm_kernel : allreduce_norm_kernel;
 }
 
-// every GEMM of the engine goes through here so that the decode step's weight-streaming launches join the
-// prefetcher's table (launch.cuh: PfCtx) without threading the context through each call site
+// every GEMM of the engine goes through here so that, without threading them through each call site, the decode
+// step's weight-streaming launches join the prefetcher's table (launch.cuh: PfCtx) and swap-AB GEMMs get the stream-K workspace
 static int launch_gemm(b200_engine* e, GemmArgs& a, int sms, cudaStream_t s) {
   a.pf = &e->pf;
+  if (a.stream_a) { a.sk_ws = e->sk_ws; a.sk_flags = e->sk_flags; a.sk_tiles = e->sk_tiles; a.sk_ws_floats = e->sk_ws_floats; }
   if (e->pf_cur && e->pf.active && pf_eligible(a) && s == e->stream) {
     // capture: beside GEMM i (it starts when its predecessor in the chain has completed) prefetch the head of GEMM i+1's
     // weight stream; after the step's last GEMM (LM head) that is the first GEMM of the next step (L2 survives the launch)
@@ -298,7 +299,7 @@ static int allreduce_bf16(b200_engine* e, bf16* buf, size_t count, cudaStream_t 
 }
 
 // ---- sparse MoE block of one layer (route, group rows per expert, expert GEMMs bounded by the device-side counts,
-// combine + residual + next RMSNorm).  forward_layers and b200_op_moe_block both launch it through here.
+// combine + residual + next RMSNorm).  moe_layer and b200_op_moe_block both launch it through here.
 enum MoeMode : int { MOE_PREFILL = 0, MOE_DECODE_GROUPED = 1, MOE_DECODE_PER_EXPERT = 2 };
 
 struct MoeBlock {
@@ -378,32 +379,210 @@ static int launch_moe_block(TmapCache& tmaps, const MoeBlock& m, int mode, int s
   return 0;
 }
 
-// ---- one transformer stack pass over T token rows --------------------------------------------------
-// decode == true : T == B rows, swap-AB GEMMs (+ split-K), flash-decoding attention
-// decode == false: packed prompt tokens, row-major GEMMs, causal flash attention
-static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, bool decode, const int32_t* kv_off = nullptr) {
-  const int H = e->H, bn = pick_block_n(B_all);
-  const float eps = e->cfg.rms_eps;
-  const float scale_log2 = (1.0f / sqrtf((float)kHeadDim)) * 1.4426950408889634f;
-  const bool tp = e->cfg.tp_size > 1;
+// row-parallel output in ybuf rows r0 .. r0 + T - 1: all-reduce (nothing to do on one GPU), residual add, next RMSNorm
+static int allreduce_norm(b200_engine* e, long long r0, int T, const bf16* next_norm, cudaStream_t s) {
+  const int H = e->H;
   int rc;
-  pdl_phase() = decode;
+  if ((rc = allreduce_bf16(e, e->ybuf + r0 * H, (size_t)T * H, s))) return rc;
+  if ((rc = launch_rmsnorm(2, e->x + r0 * H, next_norm, e->xn + r0 * H, T, H, e->cfg.rms_eps, nullptr, 0, 0, 0, e->ybuf + r0 * H, s))) return rc;
+  e->launches++;
+  return 0;
+}
+
+// decode: all-reduce over peer memory + residual + next RMSNorm in one kernel, of the row-parallel output in ybuf or,
+// when splits > 1, of its split-K partials in ws (reduced on the way)
+static int peer_allreduce_norm(b200_engine* e, int B, const bf16* next_norm, int splits, cudaStream_t s) {
+  const int H = e->H;
+  const bool part = splits > 1;
+  B200_CUDA_OK(launch_k(ar_kernel(e), dim3(B), dim3(kNormThreads), (size_t)(H + 32) * sizeof(float), s, e->p2p, e->x, next_norm,
+                        e->xn, e->cfg.rms_eps, part ? (const float*)e->ws : nullptr, part ? splits : 0, part ? (long long)B * H : 0LL,
+                        part ? (long long)H : 0LL, part ? nullptr : (const bf16*)e->ybuf, e->ar_index++, 2 * e->L));
+  e->launches++;
+  return 0;
+}
+
+// the MoE block of a layer (after o_proj), then under TP the all-reduce of the combined expert outputs + residual + next norm
+static int moe_layer(b200_engine* e, const LayerW& w, int T, const bf16* next_norm, int mode, int sms, cudaStream_t s) {
+  int rc;
+  MoeBlock mb{T, e->H, e->I, e->E, e->cfg.rms_eps, w.wr, w.wgu_e, w.wdown_e, next_norm, e->x, e->xn,
+              e->tok_expert, e->tok_weight, e->tok_row, e->e_count, e->e_off, e->xg, e->hg, e->yg, e->g_rows,
+              e->ws, mode == MOE_DECODE_PER_EXPERT ? pick_splits(e, e->H, e->I) : 1, e->cfg.tp_size > 1 ? e->ybuf : nullptr,
+              e->sk_ws, e->sk_flags, e->sk_tiles, e->sk_ws_floats};
+  // (the MoE GEMMs have device-side extents, so none of them is pf_eligible: launch_gemm(e, ...) would add nothing)
+  if ((rc = launch_moe_block(e->tmaps, mb, mode, sms, s, &e->launches))) return rc;
+  if (e->cfg.tp_size == 1) return 0;
+  if (mode != MOE_PREFILL && e->p2p_ready) return peer_allreduce_norm(e, T, next_norm, 1, s);
+  return allreduce_norm(e, 0, T, next_norm, s);
+}
+
+// decode o_proj / down_proj (split-K when it has too few tiles for the SMs) + residual + next RMSNorm
+static int decode_row_parallel(b200_engine* e, int B, const bf16* act, int K, const bf16* wmat, const uint8_t* wmat8,
+                               const bf16* wscale, const bf16* next_norm) {
+  const int H = e->H, sp = pick_splits(e, H, K);
+  const bool tp = e->cfg.tp_size > 1;
+  cudaStream_t s = e->stream;
+  int rc;
+  GemmArgs a{wmat, H, act, e->cap_T, H, B, K, sp > 1 ? EPI_T_PARTIAL : EPI_T_STORE, pick_block_n(B), sp,
+             sp > 1 ? (void*)e->ws : (void*)e->ybuf, nullptr, H, sp > 1 ? (long long)B * H : 0LL, 0, true};
+  a.a8 = wmat8; a.a_scale = wscale;
+  if ((rc = launch_gemm(e, a, e->num_sms, s))) return rc;
+  e->launches++;
+  if (sp > 1 && !tp) {
+    if ((rc = launch_rmsnorm(1, e->x, next_norm, e->xn, B, H, e->cfg.rms_eps, e->ws, sp, (long long)B * H, H, nullptr, s))) return rc;
+    e->launches++;
+    return 0;
+  }
+  if (tp && e->p2p_ready) return peer_allreduce_norm(e, B, next_norm, sp, s);
+  if (sp > 1) {
+    B200_CUDA_OK(launch_k(reduce_partials_kernel, dim3(B), dim3(256), 0, s, (const float*)e->ws, sp, (long long)B * H, (long long)H, e->ybuf, H));
+    e->launches++;
+  }
+  return allreduce_norm(e, 0, B, next_norm, s);
+}
+
+// ---- decode: one new token of each of B sequences through the stack: swap-AB GEMMs (+ split-K), flash-decoding
+// attention with RoPE + KV append fused in
+static int decode_layers(b200_engine* e, int B) {
+  const int H = e->H, bn = pick_block_n(B);
+  const float scale_log2 = (1.0f / sqrtf((float)kHeadDim)) * 1.4426950408889634f;
+  cudaStream_t s = e->stream;
+  int rc;
+  pdl_phase() = true;
   e->ar_index = 0;
-  if (!decode) e->tmaps.trim();
+  B200_CUDA_OK(launch_k(embed_gather_kernel, dim3(B), dim3(128), 0, s, (const int32_t*)e->d_next_tok, (const bf16*)e->embed, e->x, H, e->V));
+  e->launches++;
+  if ((rc = launch_rmsnorm(0, e->x, e->layers[0].ln1, e->xn, B, H, e->cfg.rms_eps, nullptr, 0, 0, 0, nullptr, s))) return rc;
+  e->launches++;
+  for (int l = 0; l < e->L; ++l) {
+    const LayerW& w = e->layers[l];
+    bf16* kc = reinterpret_cast<bf16*>(e->kcache + (long long)l * e->layer_stride);
+    bf16* vc = reinterpret_cast<bf16*>(e->vcache + (long long)l * e->layer_stride);
+    // ---- QKV projection
+    // uniform split-K with fp32 partials: the consumer kernel (attention prologue / rmsnorm) reduces them in
+    // parallel, which measured faster than finishing multi-piece tiles inside the GEMM (r01: 4.30 vs 4.62 ms/step)
+    const int sp = pick_splits(e, e->qkv_cols, H);
+    GemmArgs a{w.wqkv, e->qkv_cols, e->xn, e->cap_T, e->qkv_cols, B, H, sp > 1 ? EPI_T_PARTIAL : EPI_T_STORE, bn, sp,
+               sp > 1 ? (void*)e->ws : (void*)e->qkv, nullptr, e->qkv_cols, (long long)B * e->qkv_cols, 0, true};
+    a.bias = sp > 1 ? nullptr : w.bqkv;   // split-K: the attention prologue adds it to the summed partials
+    a.a8 = w.wqkv8; a.a_scale = w.sqkv;
+    if ((rc = launch_gemm(e, a, e->num_sms, s))) return rc;
+    e->launches++;
+    // ---- attention
+    AttnDecodeParams ap{};
+    ap.q = e->qdec; ap.ldq = e->nh * kHeadDim; ap.out = e->attn; ap.ldo = e->nh * kHeadDim;
+    ap.kcache = kc; ap.vcache = vc; ap.page_table = e->d_page_table; ap.max_pages = e->max_pages;
+    ap.seq_slot = e->d_seq_slot; ap.tok_pos = e->d_dec_pos; ap.nh = e->nh; ap.nkv = e->nkv; ap.G = e->G;
+    // one CTA per (sequence, kv head) already fills the machine at large batch; split the KV range only
+    // when there are fewer CTAs than SMs
+    const int ctas = B * e->nkv;
+    ap.splits = ctas >= e->num_sms ? 1 : std::max(1, std::min((e->num_sms + ctas - 1) / ctas, 8));
+    static const int force_splits = getenv("B200_ATTN_SPLITS") ? atoi(getenv("B200_ATTN_SPLITS")) : 0;   // (A/B)
+    if (force_splits > 0) ap.splits = std::min(force_splits, 8);
+    ap.part_o = e->part_o; ap.part_ml = e->part_ml; ap.scale_log2 = scale_log2;
+    ap.fuse_rope = 1; ap.qkv = e->qkv; ap.ld_qkv = e->qkv_cols; ap.cos_tab = e->cos_tab; ap.sin_tab = e->sin_tab;
+    ap.kcache_w = kc; ap.vcache_w = vc;
+    if (sp > 1) {
+      ap.qkv_partial = e->ws; ap.qkv_splits = sp; ap.qkv_split_stride = (long long)B * e->qkv_cols; ap.ld_qkv_partial = e->qkv_cols;
+      ap.qkv_bias = w.bqkv;
+    }
+    static const bool fold = getenv("B200_ATTN_COMBINE_KERNEL") == nullptr;   // =1: separate attn_combine_kernel (A/B)
+    ap.split_counter = fold ? e->attn_split_cnt : nullptr;
+    if ((rc = launch_attn_decode(ap, B, s, e->kv8))) return rc;
+    e->launches += (ap.splits > 1 && !ap.split_counter) ? 2 : 1;
+    if ((rc = decode_row_parallel(e, B, e->attn, e->nh * kHeadDim, w.wo, w.wo8, w.so, w.ln2))) return rc;
+    const bf16* next_norm = (l + 1 < e->L) ? e->layers[l + 1].ln1 : e->final_norm;
+    if (e->E > 0) {
+      // B200_MOE_PER_EXPERT=1: one launch per expert instead of the grouped decode launches (A/B)
+      static const bool per_expert = getenv("B200_MOE_PER_EXPERT") != nullptr;
+      if ((rc = moe_layer(e, w, B, next_norm, per_expert ? MOE_DECODE_PER_EXPERT : MOE_DECODE_GROUPED, e->num_sms, s))) return rc;
+      continue;
+    }
+    // ---- gate/up projection with the SwiGLU fused into the epilogue
+    const int gu_tiles = (2 * e->I + kGemmBlockM - 1) / kGemmBlockM;
+    static const bool gu_sk = getenv("B200_GU_STREAMK") != nullptr;
+    const int gsp = (gu_sk || gu_tiles * 4 >= e->num_sms * 3) ? 1 : pick_splits(e, 2 * e->I, H);
+    GemmArgs g{w.wgu, 2 * e->I, e->xn, e->cap_T, 2 * e->I, B, H, gsp > 1 ? EPI_T_PARTIAL : EPI_T_SWIGLU, bn, gsp,
+               gsp > 1 ? (void*)e->ws : (void*)e->hbuf, nullptr, gsp > 1 ? 2 * e->I : e->I,
+               gsp > 1 ? (long long)B * 2 * e->I : 0LL, gsp > 1 ? 0 : e->I, true};
+    g.a8 = w.wgu8; g.a_scale = w.sgu;
+    if ((rc = launch_gemm(e, g, e->num_sms, s))) return rc;
+    if (gsp > 1) {   // few tiles per GPU (tensor parallel): split-K partials + a reducing SwiGLU kernel
+      B200_CUDA_OK(launch_k(swiglu_reduce_kernel, dim3(B), dim3(512), 0, s, (const float*)e->ws, gsp, (long long)B * 2 * e->I,
+                            (long long)2 * e->I, e->hbuf, e->I));
+      e->launches++;
+    }
+    e->launches++;
+    if ((rc = decode_row_parallel(e, B, e->hbuf, e->I, w.wdown, w.wdown8, w.sdown, next_norm))) return rc;
+  }
+  B200_REQUIRE(e->ar_index == 0 || e->ar_index == 2 * e->L, "peer all-reduce count per step must be 2 per layer");
+  return 0;
+}
+
+struct PrefillPass {
+  int T, B, max_len;        // packed tokens, sequences, longest sequence of this pass
+  const int* lens;          // host [B]: tokens of each sequence in this pass (the tensor-parallel micro-batch split)
+  const int32_t* kv_off;    // device [B]: tokens of each sequence already cached (chunked prefill); nullptr: whole prompts
+};
+struct PrefillView { long long r0; int T, b0, B; cudaStream_t s; };   // micro-batch: rows from r0, sequences from b0
+
+// FP8 weights: the prefill GEMMs are compute-bound, so they run unchanged on W' = dequant(codes, scales), expanded once
+// per layer into one scratch (FP8 engines are single-GPU: one stream).  *w: layer l with its projections in that scratch.
+static int dequant_fp8_layer(b200_engine* e, int l, cudaStream_t s, LayerW* w) {
+  const LayerW& q = e->layers[l];
+  const long long H = e->H, QH = (long long)e->nh * kHeadDim, I = e->I;
+  *w = q;
+  w->wqkv = e->wdq;
+  w->wo = w->wqkv + e->qkv_cols * H;
+  w->wgu = w->wo + H * QH;
+  w->wdown = w->wgu + 2 * I * H;
+  Fp8Segs sg{};
+  sg.seg[0] = Fp8Seg{q.wqkv8, q.sqkv, w->wqkv, e->qkv_cols * H / 16, e->H};
+  sg.seg[1] = Fp8Seg{q.wo8, q.so, w->wo, H * QH / 16, (int)QH};
+  sg.seg[2] = Fp8Seg{q.wgu8, q.sgu, w->wgu, 2 * I * H / 16, e->H};
+  sg.seg[3] = Fp8Seg{q.wdown8, q.sdown, w->wdown, H * I / 16, e->I};
+  sg.n = 4;
+  int rc;
+  if ((rc = launch_dequant_fp8(sg, s))) return rc;
+  e->launches++;
+  return 0;
+}
+
+// o_proj / down_proj + residual + next RMSNorm of one micro-batch
+static int prefill_row_parallel(b200_engine* e, const PrefillView& vw, const bf16* act, int K, const bf16* wmat,
+                                const bf16* next_norm, int gsms) {
+  const int H = e->H;
+  const bool tp = e->cfg.tp_size > 1;   // one GPU: r0 == 0, and the GEMM epilogue adds the residual
+  int rc;
+  GemmArgs a{act + vw.r0 * K, e->cap_T - (int)vw.r0, wmat, H, vw.T, H, K, tp ? EPI_STORE : EPI_STORE_RES, 256, 1,
+             tp ? e->ybuf + vw.r0 * H : e->x, tp ? nullptr : e->x, H, 0, 0, false};
+  if ((rc = launch_gemm(e, a, gsms, vw.s))) return rc;
+  e->launches++;
+  if (tp) return allreduce_norm(e, vw.r0, vw.T, next_norm, vw.s);
+  if ((rc = launch_rmsnorm(0, e->x, next_norm, e->xn, vw.T, H, e->cfg.rms_eps, nullptr, 0, 0, 0, nullptr, vw.s))) return rc;
+  e->launches++;
+  return 0;
+}
+
+// ---- prefill: the packed prompt tokens through the stack, row-major GEMMs, causal flash attention
+static int prefill_layers(b200_engine* e, const PrefillPass& pp) {
+  const int H = e->H;
+  const float scale_log2 = (1.0f / sqrtf((float)kHeadDim)) * 1.4426950408889634f;
+  int rc;
+  pdl_phase() = false;
+  e->tmaps.trim();
   // Tensor-parallel prefill runs as two micro-batches (halves of the sequences = two row ranges of the packed
   // buffers) on two streams, issued layer by layer: while one half's 256 MiB all-reduce is on the wire the other
   // half's GEMMs / attention own the SMs (SURVEY.md §8e "prefill ... overlap by token-chunking").
-  struct View { long long r0; int T, b0, B; cudaStream_t s; };
-  View views[2] = {{0, T_all, 0, B_all, e->stream}, {0, 0, 0, 0, e->stream2}};
+  PrefillView views[2] = {{0, pp.T, 0, pp.B, e->stream}, {0, 0, 0, 0, e->stream2}};
   int nv = 1, gsms = e->num_sms;   // SMs the GEMM grids are sized for
   static const bool mb_off = getenv("B200_NO_PREFILL_OVERLAP") != nullptr;
   static const int mb_min_t = getenv("B200_PREFILL_OVERLAP_MIN_T") ? atoi(getenv("B200_PREFILL_OVERLAP_MIN_T")) : 2048;
-  if (!decode && tp && e->E == 0 && B_all >= 2 && T_all >= mb_min_t && !mb_off) {
-    const int b0 = B_all / 2;
+  if (e->cfg.tp_size > 1 && e->E == 0 && pp.B >= 2 && pp.T >= mb_min_t && !mb_off) {
+    const int b0 = pp.B / 2;
     long long r0 = 0;
-    for (int b = 0; b < b0; ++b) r0 += e->st.lens[b];
-    views[0] = View{0, (int)r0, 0, b0, e->stream};
-    views[1] = View{r0, (int)(T_all - r0), b0, B_all - b0, e->stream2};
+    for (int b = 0; b < b0; ++b) r0 += pp.lens[b];
+    views[0] = PrefillView{0, (int)r0, 0, b0, e->stream};
+    views[1] = PrefillView{r0, (int)(pp.T - r0), b0, pp.B - b0, e->stream2};
     nv = 2;
     // leave a few SMs to the collective: the persistent GEMM grids would otherwise wait for them tile-round after tile-round
     static const int reserve = getenv("B200_PREFILL_RESERVE_SMS") ? atoi(getenv("B200_PREFILL_RESERVE_SMS")) : 0;
@@ -413,82 +592,41 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
     B200_CUDA_OK(cudaStreamWaitEvent(e->stream2, e->ev_fork, 0));
   }
   for (int v = 0; v < nv; ++v) {
-    const View& vw = views[v];
-    B200_CUDA_OK(launch_k(embed_gather_kernel, dim3(vw.T), dim3(128), 0, vw.s, (const int32_t*)(decode ? e->d_next_tok : e->d_tok + vw.r0),
+    const PrefillView& vw = views[v];
+    B200_CUDA_OK(launch_k(embed_gather_kernel, dim3(vw.T), dim3(128), 0, vw.s, (const int32_t*)(e->d_tok + vw.r0),
                           (const bf16*)e->embed, e->x + vw.r0 * H, H, e->V));
     e->launches++;
-    if ((rc = launch_rmsnorm(0, e->x + vw.r0 * H, e->layers[0].ln1, e->xn + vw.r0 * H, vw.T, H, eps, nullptr, 0, 0, 0, nullptr, vw.s))) return rc;
+    if ((rc = launch_rmsnorm(0, e->x + vw.r0 * H, e->layers[0].ln1, e->xn + vw.r0 * H, vw.T, H, e->cfg.rms_eps, nullptr, 0, 0, 0, nullptr, vw.s))) return rc;
     e->launches++;
   }
   for (int l = 0; l < e->L; ++l)
   for (int v = 0; v < nv; ++v) {
-    const View& vw = views[v];
+    const PrefillView& vw = views[v];
     const int T = vw.T, B = vw.B;
-    const long long r0 = vw.r0;        // first row of this micro-batch in the packed activation buffers (0 in decode)
+    const long long r0 = vw.r0;        // first row of this micro-batch in the packed activation buffers
     cudaStream_t s = vw.s;
-    LayerW w = e->layers[l];   // (a copy: FP8 prefill points the bf16 matrices at the layer's dequantized scratch)
-    if (e->fp8 && !decode) {
-      // the prefill GEMMs are compute-bound: they run unchanged on W' = dequant(codes, scales), expanded once per layer
-      // into one scratch (one stream: FP8 engines are single-GPU, so there is no second micro-batch stream)
-      bf16* base = e->wdq;
-      const long long H_ = H, QH = (long long)e->nh * kHeadDim, I_ = e->I;
-      {
-        Fp8Segs sg{};
-        const LayerW& q = e->layers[l];
-        sg.seg[0] = Fp8Seg{q.wqkv8, q.sqkv, base, (long long)e->qkv_cols * H_ / 16, H};
-        sg.seg[1] = Fp8Seg{q.wo8, q.so, base + (long long)e->qkv_cols * H_, H_ * QH / 16, (int)QH};
-        sg.seg[2] = Fp8Seg{q.wgu8, q.sgu, base + (long long)e->qkv_cols * H_ + H_ * QH, 2 * I_ * H_ / 16, H};
-        sg.seg[3] = Fp8Seg{q.wdown8, q.sdown, base + (long long)e->qkv_cols * H_ + H_ * QH + 2 * I_ * H_, H_ * I_ / 16, e->I};
-        sg.n = 4;
-        if ((rc = launch_dequant_fp8(sg, s))) return rc;
-        e->launches++;
-      }
-      w.wqkv = base;
-      w.wo = base + (long long)e->qkv_cols * H_;
-      w.wgu = w.wo + H_ * QH;
-      w.wdown = w.wgu + 2 * I_ * H_;
-    }
+    LayerW w = e->layers[l];
+    if (e->fp8 && (rc = dequant_fp8_layer(e, l, s, &w))) return rc;
     // (with an FP8 KV cache the kernels' bf16 cache pointers address e4m3 codes: the kv8 instantiations read them as such)
     bf16* kc = reinterpret_cast<bf16*>(e->kcache + (long long)l * e->layer_stride);
     bf16* vc = reinterpret_cast<bf16*>(e->vcache + (long long)l * e->layer_stride);
     // ---- QKV projection
     RopeKvParams rp{};
-    bool fused_rope = false;
-    rp.ld = e->qkv_cols;
-    if (decode) {
-      // uniform split-K with fp32 partials: the consumer kernel (attention prologue / rmsnorm) reduces them in
-      // parallel, which measured faster than finishing multi-piece tiles inside the GEMM (r01: 4.30 vs 4.62 ms/step)
-      const int sp = pick_splits(e, e->qkv_cols, H);
-      GemmArgs a{w.wqkv, e->qkv_cols, e->xn, e->cap_T, e->qkv_cols, B, H, sp > 1 ? EPI_T_PARTIAL : EPI_T_STORE, bn, sp,
-                 sp > 1 ? (void*)e->ws : (void*)e->qkv, nullptr, e->qkv_cols, (long long)B * e->qkv_cols, 0, true};
-      a.sk_ws = e->sk_ws; a.sk_flags = e->sk_flags; a.sk_tiles = e->sk_tiles; a.sk_ws_floats = e->sk_ws_floats;
-      a.bias = sp > 1 ? nullptr : w.bqkv;   // split-K: the attention prologue adds it to the summed partials
-      a.a8 = w.wqkv8; a.a_scale = w.sqkv;
-      if ((rc = launch_gemm(e, a, e->num_sms, s))) return rc;
-      if (sp > 1) { rp.partial = e->ws; rp.splits = sp; rp.split_stride = (long long)B * e->qkv_cols; rp.ld_partial = e->qkv_cols; }
-      rp.qkv = e->qkv;
-      rp.q_out = e->qdec; rp.ldq = e->nh * kHeadDim;
-      rp.tok_seq = e->d_seq_slot; rp.tok_pos = e->d_dec_pos;
-    } else {
-      rp.qkv = e->qkv + r0 * e->qkv_cols;
-      rp.q_out = e->qkv + r0 * e->qkv_cols; rp.ldq = e->qkv_cols;  // in place
-      rp.tok_seq = e->d_tok_seq + r0; rp.tok_pos = e->d_tok_pos + r0;
-      rp.kcache = kc; rp.vcache = vc; rp.page_table = e->d_page_table; rp.max_pages = e->max_pages;
-      rp.cos_tab = e->cos_tab; rp.sin_tab = e->sin_tab; rp.nh = e->nh; rp.nkv = e->nkv; rp.kv8 = e->kv8;
-      // RoPE + KV append in the QKV GEMM's epilogue (the separate rope_kv_kernel pass re-read and re-wrote 750 MB per layer
-      // at 0.37 of the HBM peak); B200_NO_ROPE_FUSION=1 restores the two-kernel path
-      static const bool rope_fused = getenv("B200_NO_ROPE_FUSION") == nullptr;
-      fused_rope = rope_fused;
-      GemmArgs a{e->xn + r0 * H, e->cap_T - (int)r0, w.wqkv, e->qkv_cols, T, e->qkv_cols, H, fused_rope ? EPI_ROPE_KV : EPI_STORE, 256, 1,
-                 e->qkv + r0 * e->qkv_cols, nullptr, e->qkv_cols, 0, 0, false};
-      a.rope = &rp;
-      a.bias = w.bqkv;
-      if ((rc = launch_gemm(e, a, gsms, s))) return rc;
-    }
+    rp.qkv = e->qkv + r0 * e->qkv_cols; rp.ld = e->qkv_cols;
+    rp.q_out = e->qkv + r0 * e->qkv_cols; rp.ldq = e->qkv_cols;  // in place
+    rp.tok_seq = e->d_tok_seq + r0; rp.tok_pos = e->d_tok_pos + r0;
     rp.kcache = kc; rp.vcache = vc; rp.page_table = e->d_page_table; rp.max_pages = e->max_pages;
-    rp.cos_tab = e->cos_tab; rp.sin_tab = e->sin_tab; rp.nh = e->nh; rp.nkv = e->nkv;
+    rp.cos_tab = e->cos_tab; rp.sin_tab = e->sin_tab; rp.nh = e->nh; rp.nkv = e->nkv; rp.kv8 = e->kv8;
+    // RoPE + KV append in the QKV GEMM's epilogue (the separate rope_kv_kernel pass re-read and re-wrote 750 MB per layer
+    // at 0.37 of the HBM peak); B200_NO_ROPE_FUSION=1 restores the two-kernel path
+    static const bool rope_fused = getenv("B200_NO_ROPE_FUSION") == nullptr;
+    GemmArgs a{e->xn + r0 * H, e->cap_T - (int)r0, w.wqkv, e->qkv_cols, T, e->qkv_cols, H, rope_fused ? EPI_ROPE_KV : EPI_STORE, 256, 1,
+               e->qkv + r0 * e->qkv_cols, nullptr, e->qkv_cols, 0, 0, false};
+    a.rope = &rp;
+    a.bias = w.bqkv;
+    if ((rc = launch_gemm(e, a, gsms, s))) return rc;
     e->launches++;
-    if (!decode && !fused_rope) {   // decode: RoPE + KV append are fused into attn_decode_kernel
+    if (!rope_fused) {
       rp.T = T; rp.tokens_per_cta = 1;   // (4 tokens per CTA measured SLOWER: 446 vs 312 us per launch, r02 ncu)
       const dim3 grid((T + rp.tokens_per_cta - 1) / rp.tokens_per_cta);
       if (e->kv8) B200_CUDA_OK(launch_k(rope_kv_kernel<true>, grid, dim3(512), 0, s, rp));
@@ -496,152 +634,35 @@ static int forward_layers(b200_engine* e, int T_all, int B_all, int max_len, boo
       e->launches++;
     }
     // ---- attention
-    if (decode) {
-      AttnDecodeParams ap{};
-      ap.q = e->qdec; ap.ldq = e->nh * kHeadDim; ap.out = e->attn; ap.ldo = e->nh * kHeadDim;
-      ap.kcache = kc; ap.vcache = vc; ap.page_table = e->d_page_table; ap.max_pages = e->max_pages;
-      ap.seq_slot = e->d_seq_slot; ap.tok_pos = e->d_dec_pos; ap.nh = e->nh; ap.nkv = e->nkv; ap.G = e->G;
-      // one CTA per (sequence, kv head) already fills the machine at large batch; split the KV range only
-      // when there are fewer CTAs than SMs
-      const int ctas = B * e->nkv;
-      ap.splits = ctas >= e->num_sms ? 1 : std::max(1, std::min((e->num_sms + ctas - 1) / ctas, 8));
-      static const int force_splits = getenv("B200_ATTN_SPLITS") ? atoi(getenv("B200_ATTN_SPLITS")) : 0;   // (A/B)
-      if (force_splits > 0) ap.splits = std::min(force_splits, 8);
-      ap.part_o = e->part_o; ap.part_ml = e->part_ml; ap.scale_log2 = scale_log2;
-      ap.fuse_rope = 1; ap.qkv = rp.qkv; ap.ld_qkv = rp.ld; ap.qkv_partial = rp.partial; ap.qkv_splits = rp.splits;
-      ap.qkv_split_stride = rp.split_stride; ap.ld_qkv_partial = rp.ld_partial; ap.cos_tab = e->cos_tab; ap.sin_tab = e->sin_tab;
-      ap.qkv_bias = rp.partial ? w.bqkv : nullptr;
-      ap.kcache_w = kc; ap.vcache_w = vc;
-      static const bool fold = getenv("B200_ATTN_COMBINE_KERNEL") == nullptr;   // =1: separate attn_combine_kernel (A/B)
-      ap.split_counter = fold ? e->attn_split_cnt : nullptr;
-      if ((rc = launch_attn_decode(ap, B, s, e->kv8))) return rc;
-      e->launches += (ap.splits > 1 && !ap.split_counter) ? 2 : 1;
+    AttnPrefillParams ap{};
+    ap.q = e->qkv; ap.ldq = e->qkv_cols; ap.out = e->attn; ap.ldo = e->nh * kHeadDim;
+    ap.kcache = kc; ap.vcache = vc; ap.page_table = e->d_page_table; ap.max_pages = e->max_pages;
+    ap.cu_seqlens = e->d_cu + vw.b0; ap.seq_slot = e->d_seq_slot + vw.b0; ap.nh = e->nh; ap.nkv = e->nkv; ap.scale_log2 = scale_log2;
+    static const bool attn_mma = getenv("B200_ATTN_MMA") != nullptr;   // legacy mma.sync kernel for A/B runs
+    if (attn_mma) {
+      B200_REQUIRE(pp.kv_off == nullptr, "chunked prefill / prefix reuse needs the wgmma attention kernel (unset B200_ATTN_MMA)");
+      if ((rc = launch_attn_prefill(ap, B, pp.max_len, s))) return rc;
     } else {
-      AttnPrefillParams ap{};
-      ap.q = e->qkv; ap.ldq = e->qkv_cols; ap.out = e->attn; ap.ldo = e->nh * kHeadDim;
-      ap.kcache = kc; ap.vcache = vc; ap.page_table = e->d_page_table; ap.max_pages = e->max_pages;
-      ap.cu_seqlens = e->d_cu + vw.b0; ap.seq_slot = e->d_seq_slot + vw.b0; ap.nh = e->nh; ap.nkv = e->nkv; ap.scale_log2 = scale_log2;
-      static const bool attn_mma = getenv("B200_ATTN_MMA") != nullptr;   // legacy mma.sync kernel for A/B runs
-      if (attn_mma) {
-        B200_REQUIRE(kv_off == nullptr, "chunked prefill / prefix reuse needs the wgmma attention kernel (unset B200_ATTN_MMA)");
-        if ((rc = launch_attn_prefill(ap, B, max_len, s))) return rc;
-      } else {
-        AttnTcParams tp_{};
-        tp_.out = e->attn; tp_.ldo = e->nh * kHeadDim; tp_.page_table = e->d_page_table; tp_.max_pages = e->max_pages;
-        tp_.cu_seqlens = e->d_cu + vw.b0; tp_.seq_slot = e->d_seq_slot + vw.b0; tp_.nh = e->nh; tp_.nkv = e->nkv; tp_.scale_log2 = scale_log2;
-        tp_.kv_off = kv_off ? kv_off + vw.b0 : nullptr;
-        if ((rc = launch_attn_prefill_tc(e->tmaps, e->qkv, e->cap_T, e->qkv_cols, kc, vc, e->num_pages, tp_, B, max_len, s, e->kv8)))
-          return rc;
-      }
-      e->launches++;
+      AttnTcParams tp_{};
+      tp_.out = e->attn; tp_.ldo = e->nh * kHeadDim; tp_.page_table = e->d_page_table; tp_.max_pages = e->max_pages;
+      tp_.cu_seqlens = e->d_cu + vw.b0; tp_.seq_slot = e->d_seq_slot + vw.b0; tp_.nh = e->nh; tp_.nkv = e->nkv; tp_.scale_log2 = scale_log2;
+      tp_.kv_off = pp.kv_off ? pp.kv_off + vw.b0 : nullptr;
+      if ((rc = launch_attn_prefill_tc(e->tmaps, e->qkv, e->cap_T, e->qkv_cols, kc, vc, e->num_pages, tp_, B, pp.max_len, s, e->kv8)))
+        return rc;
     }
-    // ---- row-parallel projections (o_proj, down_proj) followed by residual add + next RMSNorm
-    auto row_parallel = [&](const bf16* act, int K, const bf16* wmat, const uint8_t* wmat8, const bf16* wscale,
-                            const bf16* next_norm) -> int {
-      int rc2;
-      if (decode) {
-        const int sp = pick_splits(e, H, K);
-        if (sp > 1) {
-          GemmArgs a{wmat, H, act, e->cap_T, H, B, K, EPI_T_PARTIAL, bn, sp, e->ws, nullptr, H, (long long)B * H, 0, true};
-          a.a8 = wmat8; a.a_scale = wscale;
-          if ((rc2 = launch_gemm(e, a, e->num_sms, s))) return rc2;
-          e->launches++;
-          if (!tp) {
-            if ((rc2 = launch_rmsnorm(1, e->x, next_norm, e->xn, T, H, eps, e->ws, sp, (long long)B * H, H, nullptr, s))) return rc2;
-            e->launches++;
-            return 0;
-          }
-          if (e->p2p_ready) {   // split-K reduce + all-reduce over peer memory + residual + RMSNorm in one kernel
-            B200_CUDA_OK(launch_k(ar_kernel(e), dim3(T), dim3(kNormThreads), (size_t)(H + 32) * sizeof(float), s, e->p2p,
-                                  e->x, next_norm, e->xn, eps, (const float*)e->ws, sp, (long long)B * H, (long long)H, (const bf16*)nullptr,
-                                  e->ar_index++, 2 * e->L));
-            e->launches++;
-            return 0;
-          }
-          B200_CUDA_OK(launch_k(reduce_partials_kernel, dim3(T), dim3(256), 0, s, (const float*)e->ws, sp, (long long)B * H, (long long)H, e->ybuf, H));
-          e->launches++;
-        } else {
-          GemmArgs a{wmat, H, act, e->cap_T, H, B, K, EPI_T_STORE, bn, 1, e->ybuf, nullptr, H, 0, 0, true};
-          a.sk_ws = e->sk_ws; a.sk_flags = e->sk_flags; a.sk_tiles = e->sk_tiles; a.sk_ws_floats = e->sk_ws_floats;
-          a.a8 = wmat8; a.a_scale = wscale;
-          if ((rc2 = launch_gemm(e, a, e->num_sms, s))) return rc2;
-          e->launches++;
-          if (tp && e->p2p_ready) {
-            B200_CUDA_OK(launch_k(ar_kernel(e), dim3(T), dim3(kNormThreads), (size_t)(H + 32) * sizeof(float), s, e->p2p,
-                                  e->x, next_norm, e->xn, eps, (const float*)nullptr, 0, 0LL, 0LL, (const bf16*)e->ybuf,
-                                  e->ar_index++, 2 * e->L));
-            e->launches++;
-            return 0;
-          }
-        }
-      } else {
-        if (!tp) {
-          GemmArgs a{act, e->cap_T, wmat, H, T, H, K, EPI_STORE_RES, 256, 1, e->x, e->x, H, 0, 0, false};   // (r0 == 0: one GPU)
-          if ((rc2 = launch_gemm(e, a, gsms, s))) return rc2;
-          if ((rc2 = launch_rmsnorm(0, e->x, next_norm, e->xn, T, H, eps, nullptr, 0, 0, 0, nullptr, s))) return rc2;
-          e->launches += 2;
-          return 0;
-        }
-        GemmArgs a{act + r0 * K, e->cap_T - (int)r0, wmat, H, T, H, K, EPI_STORE, 256, 1, e->ybuf + r0 * H, nullptr, H, 0, 0, false};
-        if ((rc2 = launch_gemm(e, a, gsms, s))) return rc2;
-        e->launches++;
-      }
-      if ((rc2 = allreduce_bf16(e, e->ybuf + r0 * H, (size_t)T * H, s))) return rc2;
-      if ((rc2 = launch_rmsnorm(2, e->x + r0 * H, next_norm, e->xn + r0 * H, T, H, eps, nullptr, 0, 0, 0, e->ybuf + r0 * H, s))) return rc2;
-      e->launches++;
-      return 0;
-    };
-    if ((rc = row_parallel(e->attn, e->nh * kHeadDim, w.wo, w.wo8, w.so, w.ln2))) return rc;
+    e->launches++;
+    if ((rc = prefill_row_parallel(e, vw, e->attn, e->nh * kHeadDim, w.wo, w.ln2, gsms))) return rc;
     const bf16* next_norm = (l + 1 < e->L) ? e->layers[l + 1].ln1 : e->final_norm;
     if (e->E > 0) {
-      // B200_MOE_PER_EXPERT=1: one launch per expert instead of the grouped decode launches (A/B)
-      static const bool per_expert = getenv("B200_MOE_PER_EXPERT") != nullptr;
-      const int mode = !decode ? MOE_PREFILL : (per_expert ? MOE_DECODE_PER_EXPERT : MOE_DECODE_GROUPED);
-      MoeBlock mb{T, H, e->I, e->E, eps, w.wr, w.wgu_e, w.wdown_e, next_norm, e->x, e->xn,
-                  e->tok_expert, e->tok_weight, e->tok_row, e->e_count, e->e_off, e->xg, e->hg, e->yg, e->g_rows,
-                  e->ws, mode == MOE_DECODE_PER_EXPERT ? pick_splits(e, H, e->I) : 1, tp ? e->ybuf : nullptr,
-                  e->sk_ws, e->sk_flags, e->sk_tiles, e->sk_ws_floats};
-      // (the MoE GEMMs have device-side extents, so none of them is pf_eligible: launch_gemm(e, ...) would add nothing)
-      if ((rc = launch_moe_block(e->tmaps, mb, mode, decode ? e->num_sms : gsms, s, &e->launches))) return rc;
-      if (tp && decode && e->p2p_ready) {   // all-reduce of the combined expert outputs + residual + next norm, over peer memory
-        B200_CUDA_OK(launch_k(ar_kernel(e), dim3(T), dim3(kNormThreads), (size_t)(H + 32) * sizeof(float), s, e->p2p,
-                              e->x, next_norm, e->xn, eps, (const float*)nullptr, 0, 0LL, 0LL, (const bf16*)e->ybuf,
-                              e->ar_index++, 2 * e->L));
-        e->launches++;
-      } else if (tp) {
-        if ((rc = allreduce_bf16(e, e->ybuf, (size_t)T * H, s))) return rc;
-        if ((rc = launch_rmsnorm(2, e->x, next_norm, e->xn, T, H, eps, nullptr, 0, 0, 0, e->ybuf, s))) return rc;
-        e->launches++;
-      }
+      if ((rc = moe_layer(e, w, T, next_norm, MOE_PREFILL, gsms, s))) return rc;
       continue;
     }
     // ---- gate/up projection with the SwiGLU fused into the epilogue
-    if (decode) {
-      const int gu_tiles = (2 * e->I + kGemmBlockM - 1) / kGemmBlockM;
-      static const bool gu_sk = getenv("B200_GU_STREAMK") != nullptr;
-      const int gsp = (gu_sk || gu_tiles * 4 >= e->num_sms * 3) ? 1 : pick_splits(e, 2 * e->I, H);
-      if (gsp > 1) {   // few tiles per GPU (tensor parallel): split-K partials + a reducing SwiGLU kernel
-        GemmArgs a{w.wgu, 2 * e->I, e->xn, e->cap_T, 2 * e->I, B, H, EPI_T_PARTIAL, bn, gsp, e->ws, nullptr, 2 * e->I,
-                   (long long)B * 2 * e->I, 0, true};
-        a.a8 = w.wgu8; a.a_scale = w.sgu;
-        if ((rc = launch_gemm(e, a, e->num_sms, s))) return rc;
-        B200_CUDA_OK(launch_k(swiglu_reduce_kernel, dim3(B), dim3(512), 0, s, (const float*)e->ws, gsp, (long long)B * 2 * e->I,
-                              (long long)2 * e->I, e->hbuf, e->I));
-        e->launches++;
-      } else {
-        GemmArgs a{w.wgu, 2 * e->I, e->xn, e->cap_T, 2 * e->I, B, H, EPI_T_SWIGLU, bn, 1, e->hbuf, nullptr, e->I, 0, e->I, true};
-        a.sk_ws = e->sk_ws; a.sk_flags = e->sk_flags; a.sk_tiles = e->sk_tiles; a.sk_ws_floats = e->sk_ws_floats;
-        a.a8 = w.wgu8; a.a_scale = w.sgu;
-        if ((rc = launch_gemm(e, a, e->num_sms, s))) return rc;
-      }
-    } else {
-      GemmArgs a{e->xn + r0 * H, e->cap_T - (int)r0, w.wgu, 2 * e->I, T, 2 * e->I, H, EPI_SWIGLU, 256, 1, e->hbuf + r0 * e->I, nullptr, e->I, 0, e->I, false};
-      if ((rc = launch_gemm(e, a, gsms, s))) return rc;
-    }
+    GemmArgs g{e->xn + r0 * H, e->cap_T - (int)r0, w.wgu, 2 * e->I, T, 2 * e->I, H, EPI_SWIGLU, 256, 1, e->hbuf + r0 * e->I, nullptr, e->I, 0, e->I, false};
+    if ((rc = launch_gemm(e, g, gsms, s))) return rc;
     e->launches++;
-    if ((rc = row_parallel(e->hbuf, e->I, w.wdown, w.wdown8, w.sdown, next_norm))) return rc;
+    if ((rc = prefill_row_parallel(e, vw, e->hbuf, e->I, w.wdown, next_norm, gsms))) return rc;
   }
-  B200_REQUIRE(e->ar_index == 0 || e->ar_index == 2 * e->L, "peer all-reduce count per step must be 2 per layer");
   if (nv == 2) {
     B200_CUDA_OK(cudaEventRecord(e->ev_join, e->stream2));
     B200_CUDA_OK(cudaStreamWaitEvent(e->stream, e->ev_join, 0));
@@ -655,7 +676,6 @@ static int head_and_step(b200_engine* e, const bf16* rows_xn, int rows_cap, int 
   int rc;
   GemmArgs a{e->lm_head, e->Vl, rows_xn, rows_cap, e->Vl, B, e->H, EPI_T_STORE, pick_block_n(B), 1,
              e->logits, nullptr, e->Vl, 0, 0, true};
-  a.sk_ws = e->sk_ws; a.sk_flags = e->sk_flags; a.sk_tiles = e->sk_tiles; a.sk_ws_floats = e->sk_ws_floats;
   if ((rc = launch_gemm(e, a, e->num_sms, s))) return rc;
   const int use_p2p = (e->cfg.tp_size > 1 && e->p2p_ready) ? 1 : 0;
   // one GPU: 16 CTAs per row scan slices of the 128k-entry row (a single CTA per row took 65 us of the 4.3 ms step)
@@ -711,7 +731,7 @@ static int prefill(b200_engine* e) {
     B200_CUDA_OK(cudaGetLastError());
     e->launches++;
   }
-  if ((rc = forward_layers(e, st.T, st.B, st.max_len, false))) return rc;
+  if ((rc = prefill_layers(e, PrefillPass{st.T, st.B, st.max_len, st.lens.data(), nullptr}))) return rc;
   B200_CUDA_OK(launch_k(gather_rows_kernel, dim3(st.B), dim3(128), 0, e->stream, (const bf16*)e->xn, (const int32_t*)e->d_last_rows, e->xl, e->H));
   e->launches++;
   return head_and_step(e, e->xl, e->rows_cap, st.B);
@@ -719,7 +739,7 @@ static int prefill(b200_engine* e) {
 
 static int decode_step_enqueue(b200_engine* e) {
   int rc;
-  if ((rc = forward_layers(e, e->st.B, e->st.B, 0, true))) return rc;
+  if ((rc = decode_layers(e, e->st.B))) return rc;
   return head_and_step(e, e->xn, e->cap_T, e->st.B);
 }
 
@@ -992,7 +1012,7 @@ static int cb_decode_enqueue(b200_engine* e, int R) {
   B200_CUDA_OK(launch_k(cb_gather_kernel, dim3(1), dim3(64), 0, e->stream, (const int32_t*)e->d_cb_row_slot, R, e->cb, e->d_next_tok,
                         e->d_seq_slot, e->d_dec_pos));
   e->launches++;
-  if ((rc = forward_layers(e, R, R, 0, true))) return rc;
+  if ((rc = decode_layers(e, R))) return rc;
   return head_and_step(e, e->xn, e->cap_T, R, e->d_cb_row_slot);
 }
 
@@ -1104,8 +1124,7 @@ static int cb_prefill_pending(b200_engine* e, long long budget) {
     B200_CUDA_OK(cudaMemcpyAsync(e->d_cb_rec, h_fin, (size_t)nfin * 4, cudaMemcpyHostToDevice, s));   // row -> slot of the finishing rows
   }
   int rc;
-  e->st.lens = lens;
-  if ((rc = forward_layers(e, T, n, max_len, false, e->d_kv_off))) return rc;
+  if ((rc = prefill_layers(e, PrefillPass{T, n, max_len, lens.data(), e->d_kv_off}))) return rc;
   if (nfin) {
     B200_CUDA_OK(launch_k(gather_rows_kernel, dim3(nfin), dim3(128), 0, s, (const bf16*)e->xn, (const int32_t*)e->d_last_rows, e->xl, e->H));
     e->launches++;
