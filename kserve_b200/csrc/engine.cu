@@ -68,12 +68,6 @@ struct Nccl {
     }                                                                                       \
   } while (0)
 
-template <class T>
-static int dmalloc(T** p, size_t n) {
-  B200_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T)));
-  return 0;
-}
-
 struct LayerW {
   bf16 *wqkv = nullptr, *wo = nullptr, *wgu = nullptr, *wdown = nullptr, *ln1 = nullptr, *ln2 = nullptr;
   bf16 *wr = nullptr, *wgu_e = nullptr, *wdown_e = nullptr;   // MoE: router [E][H], experts [E][2I][H] / [E][H][I]
@@ -89,7 +83,10 @@ struct LayerW {
 using namespace b200;
 
 struct b200_engine {
+  ~b200_engine();
   b200_model_config_t cfg;
+  // every device / pinned allocation the engine owns (dmalloc / hmalloc), released by the destructor
+  std::vector<void*> dev_allocs, host_allocs;
   int num_sms = 132;
   cudaStream_t stream = nullptr;
   cudaStream_t stream2 = nullptr;            // second micro-batch of a tensor-parallel prefill
@@ -180,7 +177,6 @@ struct b200_engine {
   int ar_index = 0;   // index of the next peer all-reduce inside the forward pass being recorded
   int big_epoch[2] = {0, 0};   // prefill all-reduce epochs, one per micro-batch stream (identical on every rank)
   int* big_cnt = nullptr;      // [2] CTA arrival counters of allreduce_big_kernel
-  bool ybuf_in_block = false;  // ybuf lives inside the IPC-shared exchange block (tp > 1)
   bool p2p_ready = false;
   P2P p2p{};
   b200_timing_t timing{};
@@ -234,6 +230,46 @@ struct b200_engine {
 };
 
 namespace b200 {
+
+template <class T>
+static int dmalloc(b200_engine* e, T** p, size_t n) {
+  B200_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T)));
+  e->dev_allocs.push_back(*p);
+  return 0;
+}
+
+template <class T>
+static int hmalloc(b200_engine* e, T** p, size_t n) {
+  B200_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(p), n * sizeof(T)));
+  e->host_allocs.push_back(*p);
+  return 0;
+}
+
+// the [max_batch][seen_words] token-presence bitmaps, allocated on first use and zero when this returns (callers then
+// write single rows with synchronous copies, which are not ordered after the engine stream)
+static int ensure_seen(b200_engine* e) {
+  if (e->d_seen) return 0;
+  const int words = (e->Vl + 31) / 32;
+  int rc;
+  if ((rc = dmalloc(e, &e->d_seen, (size_t)e->cfg.max_batch * words))) return rc;
+  e->seen_words = words;
+  B200_CUDA_OK(cudaMemsetAsync(e->d_seen, 0, (size_t)e->cfg.max_batch * words * 4, e->stream));
+  B200_CUDA_OK(cudaStreamSynchronize(e->stream));
+  return 0;
+}
+
+// pinned host buffer of at least `bytes` for the KV pages of a swapped-out slot; kept for the slot's next swap-out
+static int host_kv_reserve(b200_engine* e, int slot, size_t bytes) {
+  if (e->host_kv.count(slot)) {
+    if (e->host_kv_bytes[slot] >= bytes) return 0;
+    cudaFreeHost(e->host_kv[slot]);
+    e->host_kv.erase(slot);   // a failed allocation below must not leave the freed buffer behind
+  }
+  bf16* h = nullptr;
+  B200_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&h), bytes));
+  e->host_kv[slot] = h; e->host_kv_bytes[slot] = bytes;
+  return 0;
+}
 
 constexpr int kMaxRows = 64;   // rows of one decode / LM-head pass (swap-AB GEMM block_n, peer-exchange rows)
 static int pick_block_n(int B) { return B <= 16 ? 16 : (B <= 32 ? 32 : 64); }
@@ -879,12 +915,10 @@ static int stage_common(b200_engine* e, int B, int S, const std::vector<int>& le
   st.sample_on = st.rep_on || sc.do_sample;
   if (st.sample_on) {
     B200_REQUIRE(e->cfg.tp_size == 1, "logits processors / sampling run on one GPU per engine (tp_size == 1)");
-    if (!e->d_sample_cfg) B200_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&e->d_sample_cfg), sizeof(SampleCfg)));
+    int rc;
+    if (!e->d_sample_cfg && (rc = dmalloc(e, &e->d_sample_cfg, 1))) return rc;
     B200_CUDA_OK(cudaMemcpy(e->d_sample_cfg, &sc, sizeof(sc), cudaMemcpyHostToDevice));
-    if (st.rep_on && !e->d_seen) {
-      e->seen_words = (e->Vl + 31) / 32;
-      B200_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&e->d_seen), (size_t)e->cfg.max_batch * e->seen_words * 4));
-    }
+    if (st.rep_on && (rc = ensure_seen(e))) return rc;
   }
   return 0;
 }
@@ -988,23 +1022,22 @@ static int cb_alloc(b200_engine* e) {
   if (e->cb.len) return 0;
   const size_t nb = (size_t)e->cfg.max_batch;
   int rc;
-  if ((rc = dmalloc(&e->cb.len, nb))) return rc;
-  if ((rc = dmalloc(&e->cb.n_gen, nb))) return rc;
-  if ((rc = dmalloc(&e->cb.max_new, nb))) return rc;
-  if ((rc = dmalloc(&e->cb.finished, nb))) return rc;
-  if ((rc = dmalloc(&e->cb.stop_hit, nb))) return rc;
-  if ((rc = dmalloc(&e->cb.next_tok, nb))) return rc;
-  if ((rc = dmalloc(&e->cb.stop_len, nb * kCbMaxStop))) return rc;
-  if ((rc = dmalloc(&e->cb.stop_tok, nb * kCbMaxStop * kCbMaxStopLen))) return rc;
-  if ((rc = dmalloc(&e->d_cb_row_slot, nb))) return rc;
-  if ((rc = dmalloc(&e->d_cb_rec, nb * kCbInitInts))) return rc;
-  if ((rc = dmalloc(&e->d_cb_cfg, nb))) return rc;
-  if ((rc = dmalloc(&e->d_kv_off, (size_t)80))) return rc;
+  if ((rc = dmalloc(e, &e->cb.len, nb))) return rc;
+  if ((rc = dmalloc(e, &e->cb.n_gen, nb))) return rc;
+  if ((rc = dmalloc(e, &e->cb.max_new, nb))) return rc;
+  if ((rc = dmalloc(e, &e->cb.finished, nb))) return rc;
+  if ((rc = dmalloc(e, &e->cb.stop_hit, nb))) return rc;
+  if ((rc = dmalloc(e, &e->cb.next_tok, nb))) return rc;
+  if ((rc = dmalloc(e, &e->cb.stop_len, nb * kCbMaxStop))) return rc;
+  if ((rc = dmalloc(e, &e->cb.stop_tok, nb * kCbMaxStop * kCbMaxStopLen))) return rc;
+  if ((rc = dmalloc(e, &e->d_cb_row_slot, nb))) return rc;
+  if ((rc = dmalloc(e, &e->d_cb_rec, nb * kCbInitInts))) return rc;
+  if ((rc = dmalloc(e, &e->d_cb_cfg, nb))) return rc;
+  if ((rc = dmalloc(e, &e->d_kv_off, (size_t)80))) return rc;
   e->cb.out = e->d_out_tokens; e->cb.out_ld = e->out_ld;
   const size_t host_ints = std::max(nb * kCbInitInts, std::max((size_t)e->out_ld, 4 * nb));
-  B200_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&e->h_cb), host_ints * 4));
-  B200_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&e->h_cb_rows), (size_t)8 * kMaxRows * 4));
-  return 0;
+  if ((rc = hmalloc(e, &e->h_cb, host_ints))) return rc;
+  return hmalloc(e, &e->h_cb_rows, (size_t)8 * kMaxRows);
 }
 
 static int cb_decode_enqueue(b200_engine* e, int R) {
@@ -1260,16 +1293,14 @@ static int cb_admit(b200_engine* e, int n, const int64_t* const* rows, const int
   cb_init_kernel<<<n, 64, 0, s>>>(e->d_cb_rec, n, e->cb);
   B200_CUDA_OK(cudaGetLastError());
   // ---- logits processors / sampling per sequence (build_generation_config, generative_model.py:388-402)
+  int rc;
   for (int i = 0; i < n; ++i) {
     const SampleCfg sc = sample_cfg(sampling ? sampling + i : nullptr);
     const bool on = sc.rep_penalty != 1.0f || sc.do_sample;
     if (on && e->cfg.tp_size != 1) { rollback(n); set_last_error("logits processors / sampling run on one GPU per engine (tp_size == 1)"); return -2; }
     B200_CUDA_OK(cudaMemcpyAsync(e->d_cb_cfg + slots[i], &sc, sizeof(sc), cudaMemcpyHostToDevice, s));   // (pageable source: staged before return)
     if (on && sc.rep_penalty != 1.0f) {
-      if (!e->d_seen) {
-        e->seen_words = (e->Vl + 31) / 32;
-        B200_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&e->d_seen), (size_t)e->cfg.max_batch * e->seen_words * 4));
-      }
+      if ((rc = ensure_seen(e))) return rc;
       std::vector<uint32_t> bits(e->seen_words, 0u);      // the reference's input_ids = the prompt tokens
       for (int32_t tk : plans[i].toks)
         if (tk >= 0 && tk < e->Vl) bits[tk >> 5] |= 1u << (tk & 31);
@@ -1279,11 +1310,8 @@ static int cb_admit(b200_engine* e, int n, const int64_t* const* rows, const int
     }
     if (on) { e->cb_slot_sampling[slots[i]] = 1; e->cb_sampling_slots++; }
   }
-  if (e->cb_sampling_slots > 0 && !e->d_seen) {   // the step kernel updates the bitmaps whenever the processed path is on
-    e->seen_words = (e->Vl + 31) / 32;
-    B200_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&e->d_seen), (size_t)e->cfg.max_batch * e->seen_words * 4));
-    B200_CUDA_OK(cudaMemset(e->d_seen, 0, (size_t)e->cfg.max_batch * e->seen_words * 4));
-  }
+  // the step kernel updates the bitmaps whenever the processed path is on
+  if (e->cb_sampling_slots > 0 && (rc = ensure_seen(e))) return rc;
   B200_CUDA_OK(cudaStreamSynchronize(s));   // h_cb / sc are reused
   e->cb_stat[0] += stat_prompt; e->cb_stat[1] += stat_hit;
   for (int i = 0; i < n; ++i) {
@@ -1292,10 +1320,8 @@ static int cb_admit(b200_engine* e, int n, const int64_t* const* rows, const int
     e->cb_pending.push_back(std::move(plans[i]));
   }
   if (e->cb_chunk_tokens == 0) {
-    while (!e->cb_pending.empty()) {
-      int rc = cb_prefill_pending(e, LLONG_MAX);
-      if (rc) return rc;
-    }
+    while (!e->cb_pending.empty())
+      if ((rc = cb_prefill_pending(e, LLONG_MAX))) return rc;
   }
   return 0;
 }
@@ -1368,7 +1394,8 @@ int b200_engine_create(const b200_model_config_t* c, const void* nccl_id, b200_e
   B200_CUDA_OK(cudaGetDeviceProperties(&prop, c->device));
   B200_REQUIRE(prop.major == 9 && prop.minor == 0, std::string("kserve_b200 kernels are built for sm_90a only; device is sm_") +
                                      std::to_string(prop.major) + std::to_string(prop.minor));
-  std::unique_ptr<b200_engine> e(new b200_engine());
+  std::unique_ptr<b200_engine> owner(new b200_engine());   // a failed create returns through ~b200_engine
+  b200_engine* e = owner.get();
   e->cfg = *c;
   e->num_sms = prop.multiProcessorCount;
   const int tp = c->tp_size;
@@ -1398,37 +1425,37 @@ int b200_engine_create(const b200_model_config_t* c, const void* nccl_id, b200_e
   int rc;
   const size_t H = e->H;
   // weights
-  if ((rc = dmalloc(&e->embed, (size_t)e->V * H))) return rc;
-  if ((rc = dmalloc(&e->lm_head, (size_t)e->Vl * H))) return rc;
-  if ((rc = dmalloc(&e->final_norm, H))) return rc;
+  if ((rc = dmalloc(e, &e->embed, (size_t)e->V * H))) return rc;
+  if ((rc = dmalloc(e, &e->lm_head, (size_t)e->Vl * H))) return rc;
+  if ((rc = dmalloc(e, &e->final_norm, H))) return rc;
   e->layers.resize(e->L);
   e->fp8 = c->weight_format == 1;
   for (auto& w : e->layers) {
     if (e->fp8) {
-      if ((rc = dmalloc(&w.wqkv8, (size_t)e->qkv_cols * H))) return rc;
-      if ((rc = dmalloc(&w.wo8, H * e->nh * kHeadDim))) return rc;
-      if ((rc = dmalloc(&w.wgu8, (size_t)2 * e->I * H))) return rc;
-      if ((rc = dmalloc(&w.wdown8, H * e->I))) return rc;
-      if ((rc = dmalloc(&w.sqkv, (size_t)e->qkv_cols))) return rc;
-      if ((rc = dmalloc(&w.so, H))) return rc;
-      if ((rc = dmalloc(&w.sgu, (size_t)2 * e->I))) return rc;
-      if ((rc = dmalloc(&w.sdown, H))) return rc;
+      if ((rc = dmalloc(e, &w.wqkv8, (size_t)e->qkv_cols * H))) return rc;
+      if ((rc = dmalloc(e, &w.wo8, H * e->nh * kHeadDim))) return rc;
+      if ((rc = dmalloc(e, &w.wgu8, (size_t)2 * e->I * H))) return rc;
+      if ((rc = dmalloc(e, &w.wdown8, H * e->I))) return rc;
+      if ((rc = dmalloc(e, &w.sqkv, (size_t)e->qkv_cols))) return rc;
+      if ((rc = dmalloc(e, &w.so, H))) return rc;
+      if ((rc = dmalloc(e, &w.sgu, (size_t)2 * e->I))) return rc;
+      if ((rc = dmalloc(e, &w.sdown, H))) return rc;
     } else {
-      if ((rc = dmalloc(&w.wqkv, (size_t)e->qkv_cols * H))) return rc;
-      if ((rc = dmalloc(&w.wo, H * e->nh * kHeadDim))) return rc;
+      if ((rc = dmalloc(e, &w.wqkv, (size_t)e->qkv_cols * H))) return rc;
+      if ((rc = dmalloc(e, &w.wo, H * e->nh * kHeadDim))) return rc;
     }
     if (e->E == 0 && !e->fp8) {
-      if ((rc = dmalloc(&w.wgu, (size_t)2 * e->I * H))) return rc;
-      if ((rc = dmalloc(&w.wdown, H * e->I))) return rc;
+      if ((rc = dmalloc(e, &w.wgu, (size_t)2 * e->I * H))) return rc;
+      if ((rc = dmalloc(e, &w.wdown, H * e->I))) return rc;
     } else if (e->E > 0) {
-      if ((rc = dmalloc(&w.wr, (size_t)e->E * H))) return rc;
-      if ((rc = dmalloc(&w.wgu_e, (size_t)e->E * 2 * e->I * H))) return rc;
-      if ((rc = dmalloc(&w.wdown_e, (size_t)e->E * H * e->I))) return rc;
+      if ((rc = dmalloc(e, &w.wr, (size_t)e->E * H))) return rc;
+      if ((rc = dmalloc(e, &w.wgu_e, (size_t)e->E * 2 * e->I * H))) return rc;
+      if ((rc = dmalloc(e, &w.wdown_e, (size_t)e->E * H * e->I))) return rc;
     }
-    if ((rc = dmalloc(&w.ln1, H))) return rc;
-    if ((rc = dmalloc(&w.ln2, H))) return rc;
+    if ((rc = dmalloc(e, &w.ln1, H))) return rc;
+    if ((rc = dmalloc(e, &w.ln2, H))) return rc;
   }
-  if (e->fp8 && (rc = dmalloc(&e->wdq, (size_t)e->qkv_cols * H + H * e->nh * kHeadDim + (size_t)3 * e->I * H))) return rc;
+  if (e->fp8 && (rc = dmalloc(e, &e->wdq, (size_t)e->qkv_cols * H + H * e->nh * kHeadDim + (size_t)3 * e->I * H))) return rc;
   // rope tables (engine default: double-precision angles; hosts that need bit parity with
   // LlamaRotaryEmbedding pass their own via b200_engine_set_rope_table)
   {
@@ -1442,8 +1469,8 @@ int b200_engine_create(const b200_model_config_t* c, const void* nccl_id, b200_e
         hs[(size_t)pos * 64 + i] = __float2bfloat16_rn(sinf(ang));
       }
     }
-    if ((rc = dmalloc(&e->cos_tab, (size_t)R * 64))) return rc;
-    if ((rc = dmalloc(&e->sin_tab, (size_t)R * 64))) return rc;
+    if ((rc = dmalloc(e, &e->cos_tab, (size_t)R * 64))) return rc;
+    if ((rc = dmalloc(e, &e->sin_tab, (size_t)R * 64))) return rc;
     B200_CUDA_OK(cudaMemcpy(e->cos_tab, hc.data(), hc.size() * 2, cudaMemcpyHostToDevice));
     B200_CUDA_OK(cudaMemcpy(e->sin_tab, hs.data(), hs.size() * 2, cudaMemcpyHostToDevice));
   }
@@ -1452,26 +1479,26 @@ int b200_engine_create(const b200_model_config_t* c, const void* nccl_id, b200_e
   e->max_pages = (c->max_seq_len + kPageTokens - 1) / kPageTokens;
   e->num_pages = c->num_kv_pages > 0 ? c->num_kv_pages : c->max_batch * e->max_pages;
   e->layer_stride = (long long)e->num_pages * e->nkv * kPageTokens * kHeadDim * (e->kv8 ? 1 : (long long)sizeof(bf16));
-  if ((rc = dmalloc(&e->kcache, (size_t)e->layer_stride * e->L))) return rc;
-  if ((rc = dmalloc(&e->vcache, (size_t)e->layer_stride * e->L))) return rc;
+  if ((rc = dmalloc(e, &e->kcache, (size_t)e->layer_stride * e->L))) return rc;
+  if ((rc = dmalloc(e, &e->vcache, (size_t)e->layer_stride * e->L))) return rc;
   B200_CUDA_OK(cudaMemset(e->kcache, 0, (size_t)e->layer_stride * e->L));
   B200_CUDA_OK(cudaMemset(e->vcache, 0, (size_t)e->layer_stride * e->L));
-  if ((rc = dmalloc(&e->d_page_table, (size_t)c->max_batch * e->max_pages))) return rc;
+  if ((rc = dmalloc(e, &e->d_page_table, (size_t)c->max_batch * e->max_pages))) return rc;
   e->h_page_table.assign((size_t)c->max_batch * e->max_pages, 0);
   // activations
   e->cap_T = std::max(c->max_prefill_tokens, 128);
   const size_t T = e->cap_T;
-  if ((rc = dmalloc(&e->x, T * H))) return rc;
-  if ((rc = dmalloc(&e->xn, T * H))) return rc;
-  if ((rc = dmalloc(&e->qkv, T * e->qkv_cols))) return rc;
-  if ((rc = dmalloc(&e->attn, T * e->nh * kHeadDim))) return rc;
-  if ((rc = dmalloc(&e->hbuf, T * e->I))) return rc;
-  if (tp == 1 && (rc = dmalloc(&e->ybuf, T * H))) return rc;   // tp > 1: inside the IPC-shared exchange block (below)
+  if ((rc = dmalloc(e, &e->x, T * H))) return rc;
+  if ((rc = dmalloc(e, &e->xn, T * H))) return rc;
+  if ((rc = dmalloc(e, &e->qkv, T * e->qkv_cols))) return rc;
+  if ((rc = dmalloc(e, &e->attn, T * e->nh * kHeadDim))) return rc;
+  if ((rc = dmalloc(e, &e->hbuf, T * e->I))) return rc;
+  if (tp == 1 && (rc = dmalloc(e, &e->ybuf, T * H))) return rc;   // tp > 1: inside the IPC-shared exchange block (below)
   e->rows_cap = std::min(c->max_batch, kMaxRows);
   const size_t RC = (size_t)e->rows_cap;
-  if ((rc = dmalloc(&e->xl, RC * H))) return rc;
-  if ((rc = dmalloc(&e->qdec, RC * e->nh * kHeadDim))) return rc;
-  if ((rc = dmalloc(&e->logits, RC * e->Vl))) return rc;
+  if ((rc = dmalloc(e, &e->xl, RC * H))) return rc;
+  if ((rc = dmalloc(e, &e->qdec, RC * e->nh * kHeadDim))) return rc;
+  if ((rc = dmalloc(e, &e->logits, RC * e->Vl))) return rc;
   B200_CUDA_OK(cudaMemset(e->x, 0, T * H * 2));
   B200_CUDA_OK(cudaMemset(e->xn, 0, T * H * 2));
   B200_CUDA_OK(cudaMemset(e->attn, 0, T * e->nh * kHeadDim * 2));
@@ -1481,76 +1508,75 @@ int b200_engine_create(const b200_model_config_t* c, const void* nccl_id, b200_e
   if (e->E) {
     e->ws_elems = std::max(e->ws_elems, (size_t)e->E * 16 * RC * e->H);
     e->g_rows = 2 * e->cap_T + 8 * e->E + 256;
-    if ((rc = dmalloc(&e->tok_expert, (size_t)2 * T))) return rc;
-    if ((rc = dmalloc(&e->tok_row, (size_t)2 * T))) return rc;
-    if ((rc = dmalloc(&e->tok_weight, (size_t)2 * T))) return rc;
-    if ((rc = dmalloc(&e->e_count, (size_t)kMaxExperts))) return rc;
-    if ((rc = dmalloc(&e->e_off, (size_t)kMaxExperts + 1))) return rc;
-    if ((rc = dmalloc(&e->xg, (size_t)e->g_rows * H))) return rc;
-    if ((rc = dmalloc(&e->hg, (size_t)e->g_rows * e->I))) return rc;
-    if ((rc = dmalloc(&e->yg, (size_t)e->g_rows * H))) return rc;
+    if ((rc = dmalloc(e, &e->tok_expert, (size_t)2 * T))) return rc;
+    if ((rc = dmalloc(e, &e->tok_row, (size_t)2 * T))) return rc;
+    if ((rc = dmalloc(e, &e->tok_weight, (size_t)2 * T))) return rc;
+    if ((rc = dmalloc(e, &e->e_count, (size_t)kMaxExperts))) return rc;
+    if ((rc = dmalloc(e, &e->e_off, (size_t)kMaxExperts + 1))) return rc;
+    if ((rc = dmalloc(e, &e->xg, (size_t)e->g_rows * H))) return rc;
+    if ((rc = dmalloc(e, &e->hg, (size_t)e->g_rows * e->I))) return rc;
+    if ((rc = dmalloc(e, &e->yg, (size_t)e->g_rows * H))) return rc;
     B200_CUDA_OK(cudaMemset(e->xg, 0, (size_t)e->g_rows * H * 2));
     B200_CUDA_OK(cudaMemset(e->hg, 0, (size_t)e->g_rows * e->I * 2));
   }
-  if ((rc = dmalloc(&e->ws, e->ws_elems))) return rc;
+  if ((rc = dmalloc(e, &e->ws, e->ws_elems))) return rc;
   e->sk_tiles = (std::max(2 * e->I, e->Vl) + kGemmBlockM - 1) / kGemmBlockM;
   e->sk_ws_floats = std::max<size_t>((size_t)e->sk_tiles * 2 * 64 * kGemmBlockM, (size_t)8 << 20);   // >= 32 MB
-  if ((rc = dmalloc(&e->sk_ws, e->sk_ws_floats))) return rc;
-  if ((rc = dmalloc(&e->sk_flags, (size_t)e->sk_tiles))) return rc;
+  if ((rc = dmalloc(e, &e->sk_ws, e->sk_ws_floats))) return rc;
+  if ((rc = dmalloc(e, &e->sk_flags, (size_t)e->sk_tiles))) return rc;
   B200_CUDA_OK(cudaMemset(e->sk_flags, 0, (size_t)e->sk_tiles * sizeof(int)));
-  if ((rc = dmalloc(&e->part_o, RC * e->nkv * 8 * e->G * kHeadDim))) return rc;
-  if ((rc = dmalloc(&e->part_ml, RC * e->nkv * 8 * e->G * 2))) return rc;
-  if ((rc = dmalloc(&e->attn_split_cnt, RC * e->nkv))) return rc;
+  if ((rc = dmalloc(e, &e->part_o, RC * e->nkv * 8 * e->G * kHeadDim))) return rc;
+  if ((rc = dmalloc(e, &e->part_ml, RC * e->nkv * 8 * e->G * 2))) return rc;
+  if ((rc = dmalloc(e, &e->attn_split_cnt, RC * e->nkv))) return rc;
   B200_CUDA_OK(cudaMemset(e->attn_split_cnt, 0, RC * e->nkv * sizeof(int)));
-  if ((rc = dmalloc(&e->cand_val, RC * 16))) return rc;
-  if ((rc = dmalloc(&e->cand_idx, RC * 16))) return rc;
-  if ((rc = dmalloc(&e->cand_val_all, RC * tp))) return rc;
-  if ((rc = dmalloc(&e->cand_idx_all, RC * tp))) return rc;
+  if ((rc = dmalloc(e, &e->cand_val, RC * 16))) return rc;
+  if ((rc = dmalloc(e, &e->cand_idx, RC * 16))) return rc;
+  if ((rc = dmalloc(e, &e->cand_val_all, RC * tp))) return rc;
+  if ((rc = dmalloc(e, &e->cand_idx_all, RC * tp))) return rc;
   // bookkeeping
   e->out_ld = c->max_seq_len;
-  if ((rc = dmalloc(&e->d_tok, T))) return rc;
-  if ((rc = dmalloc(&e->d_tok_seq, T))) return rc;
-  if ((rc = dmalloc(&e->d_tok_pos, T))) return rc;
-  if ((rc = dmalloc(&e->d_cu, 80))) return rc;
-  if ((rc = dmalloc(&e->d_seq_slot, 80))) return rc;
-  if ((rc = dmalloc(&e->d_last_rows, 80))) return rc;
-  if ((rc = dmalloc(&e->d_cur_len, 80))) return rc;
-  if ((rc = dmalloc(&e->d_next_tok, 80))) return rc;
-  if ((rc = dmalloc(&e->d_dec_pos, 80))) return rc;
-  if ((rc = dmalloc(&e->d_finished, 80))) return rc;
-  if ((rc = dmalloc(&e->d_out_tokens, (size_t)c->max_batch * e->out_ld))) return rc;
-  if ((rc = dmalloc(&e->d_forced, (size_t)c->max_batch * e->out_ld))) return rc;
-  if ((rc = dmalloc(&e->d_eos, 16))) return rc;
-  if ((rc = dmalloc(&e->d_stop_tok, 1024))) return rc;
-  if ((rc = dmalloc(&e->d_stop_off, 32))) return rc;
-  if ((rc = dmalloc(&e->d_state, 1))) return rc;
+  if ((rc = dmalloc(e, &e->d_tok, T))) return rc;
+  if ((rc = dmalloc(e, &e->d_tok_seq, T))) return rc;
+  if ((rc = dmalloc(e, &e->d_tok_pos, T))) return rc;
+  if ((rc = dmalloc(e, &e->d_cu, 80))) return rc;
+  if ((rc = dmalloc(e, &e->d_seq_slot, 80))) return rc;
+  if ((rc = dmalloc(e, &e->d_last_rows, 80))) return rc;
+  if ((rc = dmalloc(e, &e->d_cur_len, 80))) return rc;
+  if ((rc = dmalloc(e, &e->d_next_tok, 80))) return rc;
+  if ((rc = dmalloc(e, &e->d_dec_pos, 80))) return rc;
+  if ((rc = dmalloc(e, &e->d_finished, 80))) return rc;
+  if ((rc = dmalloc(e, &e->d_out_tokens, (size_t)c->max_batch * e->out_ld))) return rc;
+  if ((rc = dmalloc(e, &e->d_forced, (size_t)c->max_batch * e->out_ld))) return rc;
+  if ((rc = dmalloc(e, &e->d_eos, 16))) return rc;
+  if ((rc = dmalloc(e, &e->d_stop_tok, 1024))) return rc;
+  if ((rc = dmalloc(e, &e->d_stop_off, 32))) return rc;
+  if ((rc = dmalloc(e, &e->d_state, 1))) return rc;
   e->h_stage_elems = 3 * T + 8 * 80;
-  B200_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&e->h_stage), e->h_stage_elems * 4));
-  B200_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&e->h_state), sizeof(StepState)));
-  B200_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&e->h_out_tokens), (size_t)c->max_batch * e->out_ld * 4));
+  if ((rc = hmalloc(e, &e->h_stage, e->h_stage_elems))) return rc;
+  if ((rc = hmalloc(e, &e->h_state, 1))) return rc;
+  if ((rc = hmalloc(e, &e->h_out_tokens, (size_t)c->max_batch * e->out_ld))) return rc;
   {
     const size_t raw = (size_t)c->max_batch * c->max_seq_len;
-    if ((rc = dmalloc(&e->d_raw_ids, raw))) return rc;
-    if ((rc = dmalloc(&e->d_raw_mask, raw))) return rc;
-    if ((rc = dmalloc(&e->d_pred, raw))) return rc;
-    if ((rc = dmalloc(&e->d_flat, T))) return rc;
-    if ((rc = dmalloc(&e->d_offs, 80))) return rc;
+    if ((rc = dmalloc(e, &e->d_raw_ids, raw))) return rc;
+    if ((rc = dmalloc(e, &e->d_raw_mask, raw))) return rc;
+    if ((rc = dmalloc(e, &e->d_pred, raw))) return rc;
+    if ((rc = dmalloc(e, &e->d_flat, T))) return rc;
+    if ((rc = dmalloc(e, &e->d_offs, 80))) return rc;
     const size_t hraw = std::max(2 * raw, (T + 80) / 2 + 1);
-    B200_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&e->h_raw), hraw * 8));
-    B200_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&e->h_pred), raw * 8));
+    if ((rc = hmalloc(e, &e->h_raw, hraw))) return rc;
+    if ((rc = hmalloc(e, &e->h_pred, raw))) return rc;
   }
   if (tp > 1) {
     B200_REQUIRE(tp <= kMaxTp && kMaxRows <= kArRows, "tp_size exceeds the peer-exchange layout");
     const ArLayout lay = ArLayout::make(e->H);
     // one allocation = one IPC handle: [decode LL packets | candidate exchange | flags | prefill exchange buffer y[T][H]]
-    B200_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&e->ar_local), lay.total + T * H * sizeof(bf16)));
+    if ((rc = dmalloc(e, &e->ar_local, lay.total + T * H * sizeof(bf16)))) return rc;
     B200_CUDA_OK(cudaMemset(e->ar_local, 0, lay.total + T * H * sizeof(bf16)));
     e->ybuf = reinterpret_cast<bf16*>(e->ar_local + lay.total);
-    e->ybuf_in_block = true;
-    if ((rc = dmalloc(&e->big_cnt, (size_t)2))) return rc;
+    if ((rc = dmalloc(e, &e->big_cnt, (size_t)2))) return rc;
     B200_CUDA_OK(cudaMemset(e->big_cnt, 0, 2 * sizeof(int)));
-    if ((rc = dmalloc(&e->row_epoch, (size_t)kArRows))) return rc;
-    if ((rc = dmalloc(&e->cand_epoch, (size_t)kArRows))) return rc;
+    if ((rc = dmalloc(e, &e->row_epoch, (size_t)kArRows))) return rc;
+    if ((rc = dmalloc(e, &e->cand_epoch, (size_t)kArRows))) return rc;
     B200_CUDA_OK(cudaMemset(e->row_epoch, 0, kArRows * sizeof(int)));
     B200_CUDA_OK(cudaMemset(e->cand_epoch, 0, kArRows * sizeof(int)));
     e->p2p.tp = tp; e->p2p.rank = c->tp_rank; e->p2p.lay = lay; e->p2p.row_epoch = e->row_epoch; e->p2p.cand_epoch = e->cand_epoch;
@@ -1562,48 +1588,25 @@ int b200_engine_create(const b200_model_config_t* c, const void* nccl_id, b200_e
     B200_NCCL_OK(n.CommInitRank(&e->comm, tp, id, c->tp_rank));
   }
   B200_CUDA_OK(cudaDeviceSynchronize());
-  *out = e.release();
+  *out = owner.release();
   return 0;
 }
 
-int b200_engine_destroy(b200_engine_t* e) {
-  if (!e) return 0;
-  cudaSetDevice(e->cfg.device);
+// Errors are ignored: this also releases an engine that b200_engine_create abandoned halfway (some handles still null).
+b200_engine::~b200_engine() {
+  cudaSetDevice(cfg.device);
   cudaDeviceSynchronize();
-  for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);
-  if (e->ev_pf_fork) cudaEventDestroy(e->ev_pf_fork);
-  if (e->ev_pf_join) cudaEventDestroy(e->ev_pf_join);
-  if (e->comm) Nccl::get().CommDestroy(e->comm);
-  for (int r = 0; r < kMaxTp; ++r) if (e->ar_peer_map[r]) cudaIpcCloseMemHandle(e->ar_peer_map[r]);
-  if (e->ar_local) cudaFree(e->ar_local);
-  if (e->row_epoch) cudaFree(e->row_epoch);
-  if (e->cand_epoch) cudaFree(e->cand_epoch);
-  void* ptrs[] = {e->embed, e->lm_head, e->final_norm, e->cos_tab, e->sin_tab, e->kcache, e->vcache, e->d_page_table,
-                  e->x, e->xn, e->qkv, e->attn, e->hbuf, e->ybuf_in_block ? nullptr : (void*)e->ybuf, e->big_cnt, e->xl, e->qdec, e->logits, e->ws, e->sk_ws, e->sk_flags,
-                  e->tok_expert, e->tok_row, e->tok_weight, e->e_count, e->e_off, e->xg, e->hg, e->yg, e->part_o, e->part_ml, e->attn_split_cnt,
-                  e->cand_val, e->cand_idx, e->cand_val_all, e->cand_idx_all, e->d_tok, e->d_tok_seq, e->d_tok_pos, e->d_cu,
-                  e->d_seq_slot, e->d_last_rows, e->d_cur_len, e->d_next_tok, e->d_dec_pos, e->d_finished, e->d_out_tokens,
-                  e->d_forced, e->d_eos, e->d_stop_tok, e->d_stop_off, e->d_state};
-  for (void* p : ptrs) if (p) cudaFree(p);
-  for (auto& w : e->layers) {
-    void* lp[] = {w.wqkv, w.wo, w.wgu, w.wdown, w.ln1, w.ln2, w.wr, w.wgu_e, w.wdown_e, w.bqkv,
-                  w.wqkv8, w.wo8, w.wgu8, w.wdown8, w.sqkv, w.so, w.sgu, w.sdown};
-    for (void* p : lp) if (p) cudaFree(p);
-  }
-  if (e->wdq) cudaFree(e->wdq);
-  for (auto& kv : e->host_kv) cudaFreeHost(kv.second);
-  if (e->h_stage) cudaFreeHost(e->h_stage);
-  if (e->h_state) cudaFreeHost(e->h_state);
-  if (e->h_out_tokens) cudaFreeHost(e->h_out_tokens);
-  if (e->ev0) cudaEventDestroy(e->ev0);
-  if (e->ev1) cudaEventDestroy(e->ev1);
-  if (e->ev2) cudaEventDestroy(e->ev2);
-  if (e->d_sample_cfg) cudaFree(e->d_sample_cfg);
-  if (e->d_seen) cudaFree(e->d_seen);
-  if (e->stream2) cudaStreamDestroy(e->stream2);
-  if (e->ev_fork) cudaEventDestroy(e->ev_fork);
-  if (e->ev_join) cudaEventDestroy(e->ev_join);
-  if (e->stream) cudaStreamDestroy(e->stream);
+  for (auto& kv : graphs) cudaGraphExecDestroy(kv.second);
+  if (comm) Nccl::get().CommDestroy(comm);
+  for (void* p : ar_peer_map) if (p) cudaIpcCloseMemHandle(p);
+  for (void* p : dev_allocs) cudaFree(p);
+  for (void* p : host_allocs) cudaFreeHost(p);
+  for (auto& kv : host_kv) cudaFreeHost(kv.second);
+  for (cudaEvent_t ev : {ev_fork, ev_join, ev0, ev1, ev2, ev_pf_fork, ev_pf_join}) if (ev) cudaEventDestroy(ev);
+  for (cudaStream_t s : {stream, stream2}) if (s) cudaStreamDestroy(s);
+}
+
+int b200_engine_destroy(b200_engine_t* e) {
   delete e;
   return 0;
 }
@@ -1664,7 +1667,7 @@ int b200_engine_set_weight(b200_engine_t* e, const char* name, const void* data,
       const long long full = which == 'q' ? QH : KH, len = which == 'q' ? ql : kl;
       const long long off = which == 'q' ? 0 : (which == 'k' ? ql : ql + kl);
       B200_REQUIRE(expect(full, -1), "shape mismatch for " + n);
-      if (!w.bqkv && (rc = dmalloc(&w.bqkv, (size_t)e->qkv_cols))) return rc;
+      if (!w.bqkv && (rc = dmalloc(e, &w.bqkv, (size_t)e->qkv_cols))) return rc;
       rc = copy_rows(w.bqkv + off, src, r * len, len, 1, dev);
     } else if (rest == "self_attn.o_proj.weight") {
       B200_REQUIRE(expect(H, QH), "shape mismatch for " + n);
@@ -2028,12 +2031,8 @@ static int kv_swap(b200_engine_t* e, int32_t slot, bool out, int scrub) {
   const size_t seq_bytes = (size_t)st.per_seq_pages * page_bytes;         // per layer, per K or V
   const size_t bytes = seq_bytes * 2 * e->L;
   if (out) {
-    if (!e->host_kv.count(slot) || e->host_kv_bytes[slot] < bytes) {
-      if (e->host_kv.count(slot)) cudaFreeHost(e->host_kv[slot]);
-      bf16* h = nullptr;
-      B200_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&h), bytes));
-      e->host_kv[slot] = h; e->host_kv_bytes[slot] = bytes;
-    }
+    int rc;
+    if ((rc = host_kv_reserve(e, slot, bytes))) return rc;
   } else {
     B200_REQUIRE(e->host_kv.count(slot), "sequence is not swapped out");
   }
@@ -2201,13 +2200,8 @@ static int cb_swap(b200_engine_t* e, int32_t slot, bool out) {
     auto it = std::find(e->cb_active.begin(), e->cb_active.end(), (int)slot);
     B200_REQUIRE(it != e->cb_active.end(), "only a running sequence (prompt fully prefilled) can be swapped out");
     std::vector<int>& pages = e->cb_slot_pages[slot];
-    const size_t bytes = pages.size() * page_bytes * 2 * e->L;
-    if (!e->host_kv.count(slot) || e->host_kv_bytes[slot] < bytes) {
-      if (e->host_kv.count(slot)) cudaFreeHost(e->host_kv[slot]);
-      bf16* h = nullptr;
-      B200_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&h), bytes));
-      e->host_kv[slot] = h; e->host_kv_bytes[slot] = bytes;
-    }
+    int rc;
+    if ((rc = host_kv_reserve(e, slot, pages.size() * page_bytes * 2 * e->L))) return rc;
     unsigned char* h = reinterpret_cast<unsigned char*>(e->host_kv[slot]);
     for (size_t i = 0; i < pages.size(); ++i) {     // one strided copy per page and cache: [L] rows of page_bytes
       unsigned char* hk = h + (i * 2) * page_bytes * e->L;
