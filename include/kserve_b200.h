@@ -162,7 +162,7 @@ int b200_fetch_staged(b200_engine_t* e, int64_t* out_ids, int32_t* out_len, int3
 /* ---- batcher ----------------------------------------------------------------------------------------
  * Replaces BatchHandler.batchPredict (pkg/batcher/handler.go:99-155).  rows[i] / row_lens[i] are the token
  * ids of instance i of the formed batch (all waiting requests' instances, in arrival order); they are
- * concatenated on the device, generated as ONE batch and returned as predictions[n_rows][max_new_tokens]
+ * generated as ONE batch and returned as predictions[n_rows][max_new_tokens]
  * (instance order, rows padded with pad_token_id after *n_generated tokens), so request r's answer is rows
  * [first_r, first_r + count_r) exactly as handler.go:139-150 scatters them. */
 int b200_batch_predict(b200_engine_t* e, const int64_t* const* rows, const int32_t* row_lens, int32_t n_rows,

@@ -33,7 +33,7 @@ def main(argv=None):
     parser.add_argument("--tensor_parallel_size", type=int, default=int(os.environ.get("WORLD_SIZE", "1")))
     # the agent's flags (cmd/agent/main.go:66-68 --enable-batcher / --max-batchsize / --max-latency), same defaults
     parser.add_argument("--enable_batcher", "--enable-batcher", dest="enable_batcher", action="store_true",
-                        help="install the request batcher in front of V1 :predict (pkg/batcher), formed batches run as one device-side concat/scatter call")
+                        help="install the request batcher in front of V1 :predict (pkg/batcher), formed batches run as one engine call")
     parser.add_argument("--max-batchsize", "--max_batchsize", dest="max_batchsize", type=int, default=32)
     parser.add_argument("--max-latency", "--max_latency", dest="max_latency", type=int, default=5000)
     args, _ = parser.parse_known_args(argv)

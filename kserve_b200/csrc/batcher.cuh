@@ -1,7 +1,5 @@
-// Batcher: (1) the trigger / index bookkeeping of the Go sidecar's BatchHandler as a deterministic state
-// machine (pkg/batcher/handler.go:157-199), (2) device-side request concat (ragged rows -> packed token
-// buffers) and response scatter, replacing the JSON concat / loopback HTTP / JSON scatter of
-// BatchHandler.batchPredict (handler.go:99-155).
+// Batcher: the trigger / index bookkeeping of the Go sidecar's BatchHandler as a deterministic state machine
+// (pkg/batcher/handler.go:157-199).  A fired batch runs as one b200_batch_predict call.
 #pragma once
 #include <deque>
 #include <mutex>
@@ -55,83 +53,5 @@ struct BatcherCore {
     return n;
   }
 };
-
-// ---------------------------------------------------------------------------------------------------
-// Device-side concat.  Input: the raw request rows exactly as they arrived —
-//   padded form : ids int64 [B][S] + optional mask int64 [B][S] (left padding)      (OpenAI / V2 leg)
-//   ragged form : flat int32 tokens + per-row offsets                               (batcher leg)
-// Output: the engine's packed layout (tok, tok_seq, tok_pos, cu_seqlens, last_rows, lens...).  One CTA.
-// ---------------------------------------------------------------------------------------------------
-struct PackOut {
-  int32_t *tok, *tok_seq, *tok_pos, *cu, *seq_slot, *last_rows, *cur_len, *dec_pos, *finished;
-};
-
-__global__ void __launch_bounds__(1024)
-pack_padded_kernel(const long long* __restrict__ ids, const long long* __restrict__ mask, int B, int S, PackOut o) {
-  __shared__ int s_len[64], s_cu[65];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  for (int b = warp; b < B; b += nw) {
-    int first = S;
-    if (mask) {
-      for (int i = lane; i < S; i += 32)
-        if (mask[(long long)b * S + i] != 0) { first = i; break; }
-#pragma unroll
-      for (int d = 16; d > 0; d >>= 1) first = min(first, __shfl_xor_sync(0xffffffffu, first, d));
-    } else {
-      first = 0;
-    }
-    if (lane == 0) s_len[b] = S - first;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int t = 0;
-    for (int b = 0; b < B; ++b) { s_cu[b] = t; t += s_len[b]; }
-    s_cu[B] = t;
-  }
-  __syncthreads();
-  for (int b = threadIdx.x; b <= B; b += blockDim.x) {
-    o.cu[b] = s_cu[b];
-    if (b < B) {
-      o.seq_slot[b] = b; o.last_rows[b] = s_cu[b + 1] - 1; o.cur_len[b] = s_len[b]; o.dec_pos[b] = s_len[b];
-      o.finished[b] = 0;
-    }
-  }
-  for (int b = 0; b < B; ++b) {
-    const int len = s_len[b], first = S - len, base = s_cu[b];
-    for (int i = threadIdx.x; i < len; i += blockDim.x) {
-      o.tok[base + i] = (int32_t)ids[(long long)b * S + first + i];
-      o.tok_seq[base + i] = b;
-      o.tok_pos[base + i] = i;
-    }
-  }
-}
-
-__global__ void __launch_bounds__(1024)
-pack_ragged_kernel(const int32_t* __restrict__ flat, const int32_t* __restrict__ offs, int B, PackOut o) {
-  for (int b = threadIdx.x; b <= B; b += blockDim.x) {
-    o.cu[b] = offs[b];
-    if (b < B) {
-      const int len = offs[b + 1] - offs[b];
-      o.seq_slot[b] = b; o.last_rows[b] = offs[b + 1] - 1; o.cur_len[b] = len; o.dec_pos[b] = len; o.finished[b] = 0;
-    }
-  }
-  for (int b = 0; b < B; ++b) {
-    const int base = offs[b], len = offs[b + 1] - base;
-    for (int i = threadIdx.x; i < len; i += blockDim.x) {
-      o.tok[base + i] = flat[base + i];
-      o.tok_seq[base + i] = b;
-      o.tok_pos[base + i] = i;
-    }
-  }
-}
-
-// Response scatter: compacts out_tokens [B][ld] into predictions [B][T] int64 (one row per instance, in
-// instance order) so that every waiting request's slice is a contiguous range — the index arithmetic of
-// handler.go:139-150 done once on the device instead of per JSON element on the host.
-__global__ void scatter_predictions_kernel(const int32_t* __restrict__ out_tokens, int ld, int B, int T,
-                                           long long* __restrict__ pred) {
-  const int b = blockIdx.x;
-  for (int i = threadIdx.x; i < T; i += blockDim.x) pred[(long long)b * T + i] = out_tokens[(long long)b * ld + i];
-}
 
 }  // namespace b200

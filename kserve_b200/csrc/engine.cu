@@ -137,13 +137,10 @@ struct b200_engine {
           *d_last_rows = nullptr, *d_cur_len = nullptr, *d_next_tok = nullptr, *d_dec_pos = nullptr,
           *d_finished = nullptr, *d_out_tokens = nullptr, *d_forced = nullptr, *d_eos = nullptr,
           *d_stop_tok = nullptr, *d_stop_off = nullptr;
+  int32_t* d_row_init = nullptr;   // the staged batch's initial cur_len | dec_pos | finished, [3][kMaxRows] like the live rows
   StepState* d_state = nullptr;
   int out_ld = 0;
-  // raw request staging (device-side concat/pad)
-  long long *d_raw_ids = nullptr, *d_raw_mask = nullptr, *d_pred = nullptr;
-  int32_t *d_flat = nullptr, *d_offs = nullptr;
-  long long *h_raw = nullptr, *h_pred = nullptr;
-  // pinned staging
+  // pinned staging: the packed rows of one prefill pass (pack_prefill), then the static batch's initial rows
   int32_t* h_stage = nullptr;
   size_t h_stage_elems = 0;
   StepState* h_state = nullptr;
@@ -163,7 +160,6 @@ struct b200_engine {
   // host-DRAM KV tier: pinned copies of the pages of swapped-out sequences (slot -> buffer)
   std::unordered_map<int, bf16*> host_kv;
   std::unordered_map<int, size_t> host_kv_bytes;
-  bool staged_mask = false;
   // graphs per batch size
   std::unordered_map<int, cudaGraphExec_t> graphs;
   std::unordered_map<int, int> graph_nodes;
@@ -923,12 +919,67 @@ static int stage_common(b200_engine* e, int B, int S, const std::vector<int>& le
   return 0;
 }
 
-static PackOut pack_out(b200_engine* e) {
-  return PackOut{e->d_tok, e->d_tok_seq, e->d_tok_pos, e->d_cu, e->d_seq_slot, e->d_last_rows, e->d_cur_len, e->d_dec_pos, e->d_finished};
+// One row of a prefill pass: `count` tokens of the sequence in `slot`, from position `start` on (its first `start`
+// tokens are already in the KV cache); `last` when the row ends the prompt, so its logits select the first token.
+template <class Tok>
+struct PrefillRow { int slot; const Tok* toks; int start, count; bool last; };
+
+// Packs the rows of one prefill pass in pinned h_stage and copies them to the device: tok / tok_seq / tok_pos per
+// token, cu_seqlens and seq_slot per row, and last_rows for the rows that end their prompt.  A pass that continues
+// cached sequences also gets each row's start (d_kv_off), and one that scatters first tokens by slot the slot of
+// each ending row (d_fin_slot).
+template <class Tok>
+static int pack_prefill(b200_engine* e, const std::vector<PrefillRow<Tok>>& rows, int32_t* d_kv_off, int32_t* d_fin_slot) {
+  const int n = (int)rows.size();
+  int T = 0;
+  for (const auto& r : rows) T += r.count;
+  B200_REQUIRE(n <= kMaxRows && (size_t)(3 * T + 5 * n + 1) <= e->h_stage_elems - 3 * kMaxRows, "prompt staging buffer too small");
+  int32_t *h_tok = e->h_stage, *h_seq = h_tok + T, *h_pos = h_seq + T, *h_cu = h_pos + T, *h_slot = h_cu + n + 1,
+          *h_off = h_slot + n, *h_last = h_off + n, *h_fin = h_last + n;
+  int t = 0, f = 0;
+  for (int i = 0; i < n; ++i) {
+    const auto& r = rows[i];
+    h_cu[i] = t;
+    for (int k = 0; k < r.count; ++k, ++t) { h_tok[t] = (int32_t)r.toks[k]; h_seq[t] = r.slot; h_pos[t] = r.start + k; }
+    h_slot[i] = r.slot; h_off[i] = r.start;
+    if (r.last) { h_last[f] = t - 1; h_fin[f] = r.slot; ++f; }
+  }
+  h_cu[n] = t;
+  cudaStream_t s = e->stream;
+  B200_CUDA_OK(cudaMemcpyAsync(e->d_tok, h_tok, (size_t)T * 4, cudaMemcpyHostToDevice, s));
+  B200_CUDA_OK(cudaMemcpyAsync(e->d_tok_seq, h_seq, (size_t)T * 4, cudaMemcpyHostToDevice, s));
+  B200_CUDA_OK(cudaMemcpyAsync(e->d_tok_pos, h_pos, (size_t)T * 4, cudaMemcpyHostToDevice, s));
+  B200_CUDA_OK(cudaMemcpyAsync(e->d_cu, h_cu, (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, s));
+  B200_CUDA_OK(cudaMemcpyAsync(e->d_seq_slot, h_slot, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  if (d_kv_off) B200_CUDA_OK(cudaMemcpyAsync(d_kv_off, h_off, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  if (f) {
+    B200_CUDA_OK(cudaMemcpyAsync(e->d_last_rows, h_last, (size_t)f * 4, cudaMemcpyHostToDevice, s));
+    if (d_fin_slot) B200_CUDA_OK(cudaMemcpyAsync(d_fin_slot, h_fin, (size_t)f * 4, cudaMemcpyHostToDevice, s));
+  }
+  return 0;
 }
 
-// Padded [B][S] ids (+ left-padding mask) as they arrive on the OpenAI / V2 legs: the raw rows are copied to
-// the device once and concatenated into the packed layout by pack_padded_kernel.
+// cur_len / dec_pos / finished of the staged batch back to their values before prefill (one device-to-device copy)
+static int restore_rows(b200_engine* e) {
+  B200_CUDA_OK(cudaMemcpyAsync(e->d_cur_len, e->d_row_init, (size_t)3 * kMaxRows * 4, cudaMemcpyDeviceToDevice, e->stream));
+  return 0;
+}
+
+// A static batch: row b is the whole prompt of sequence b.  Besides the packed rows, each sequence starts decoding
+// with cur_len = dec_pos = its prompt length and finished = 0; those rows stay on the device (d_row_init), so
+// that b200_run_staged can replay the batch without copying them again.
+template <class Tok>
+static int stage_rows(b200_engine* e, const std::vector<PrefillRow<Tok>>& rows) {
+  int rc = pack_prefill(e, rows, nullptr, nullptr);
+  if (rc) return rc;
+  int32_t* init = e->h_stage + e->h_stage_elems - 3 * kMaxRows;
+  std::fill(init, init + 3 * kMaxRows, 0);
+  for (size_t b = 0; b < rows.size(); ++b) init[b] = init[kMaxRows + b] = rows[b].count;
+  B200_CUDA_OK(cudaMemcpyAsync(e->d_row_init, init, (size_t)3 * kMaxRows * 4, cudaMemcpyHostToDevice, e->stream));
+  return restore_rows(e);
+}
+
+// Padded [B][S] ids (+ left-padding mask) as they arrive on the OpenAI / V2 legs: each row without its padding.
 static int stage_prompt(b200_engine* e, const int64_t* ids, const int64_t* mask, int B, int S,
                         const b200_gen_params_t* gp) {
   B200_REQUIRE(B >= 1 && B <= e->rows_cap && S >= 1 && S <= e->cfg.max_seq_len, "bad batch shape");
@@ -944,20 +995,10 @@ static int stage_prompt(b200_engine* e, const int64_t* ids, const int64_t* mask,
   }
   int rc = stage_common(e, B, S, lens, gp);
   if (rc) return rc;
-  e->staged_mask = mask != nullptr;
   e->st.input.assign(ids, ids + (size_t)B * S);
-  cudaStream_t s = e->stream;
-  const size_t n = (size_t)B * S;
-  memcpy(e->h_raw, ids, n * 8);
-  B200_CUDA_OK(cudaMemcpyAsync(e->d_raw_ids, e->h_raw, n * 8, cudaMemcpyHostToDevice, s));
-  if (mask) {
-    memcpy(e->h_raw + n, mask, n * 8);
-    B200_CUDA_OK(cudaMemcpyAsync(e->d_raw_mask, e->h_raw + n, n * 8, cudaMemcpyHostToDevice, s));
-  }
-  pack_padded_kernel<<<1, 1024, 0, s>>>(e->d_raw_ids, mask ? e->d_raw_mask : nullptr, B, S, pack_out(e));
-  B200_CUDA_OK(cudaGetLastError());
-  e->launches++;
-  return 0;
+  std::vector<PrefillRow<int64_t>> rows(B);
+  for (int b = 0; b < B; ++b) rows[b] = {b, ids + (size_t)b * S + (S - lens[b]), 0, lens[b], true};
+  return stage_rows(e, rows);
 }
 
 // Ragged rows as the batcher hands them over (one row per instance of every waiting request).
@@ -968,21 +1009,9 @@ static int stage_ragged(b200_engine* e, const int64_t* const* rows, const int32_
   int rc = stage_common(e, B, 0, lens, gp);
   if (rc) return rc;
   e->st.input.clear();
-  int32_t* flat = reinterpret_cast<int32_t*>(e->h_raw);
-  int32_t* offs = flat + e->cap_T;
-  int t = 0;
-  for (int b = 0; b < B; ++b) {
-    offs[b] = t;
-    for (int i = 0; i < lens[b]; ++i) flat[t++] = (int32_t)rows[b][i];
-  }
-  offs[B] = t;
-  cudaStream_t s = e->stream;
-  B200_CUDA_OK(cudaMemcpyAsync(e->d_flat, flat, (size_t)t * 4, cudaMemcpyHostToDevice, s));
-  B200_CUDA_OK(cudaMemcpyAsync(e->d_offs, offs, (size_t)(B + 1) * 4, cudaMemcpyHostToDevice, s));
-  pack_ragged_kernel<<<1, 1024, 0, s>>>(e->d_flat, e->d_offs, B, pack_out(e));
-  B200_CUDA_OK(cudaGetLastError());
-  e->launches++;
-  return 0;
+  std::vector<PrefillRow<int64_t>> packed(B);
+  for (int b = 0; b < B; ++b) packed[b] = {b, rows[b], 0, lens[b], true};
+  return stage_rows(e, packed);
 }
 
 // called right after a stream synchronisation: did any wait of the kernels just run give up?
@@ -1016,6 +1045,75 @@ static int fetch_result(b200_engine* e, int64_t* out_ids, int32_t* out_len, int3
   return 0;
 }
 
+
+// A static batch from staging to result: `stage` packs the prompt, then prefill, decode steps until every row is done or
+// has `max_new` tokens, and the result as fetch_result writes it.  `logits_bf16` receives every step's logits (the decode
+// steps then run without the graph), `cb` is called with every step's tokens.
+template <class Stage>
+static int generate(b200_engine* e, Stage&& stage, int max_new, uint16_t* logits_bf16, b200_token_callback cb, void* user,
+                    int64_t* out_ids, int32_t* out_len, int32_t* stop_triggered) {
+  cudaStream_t s = e->stream;
+  e->launches = 0;
+  B200_CUDA_OK(cudaEventRecord(e->ev0, s));
+  int rc = stage();
+  if (rc) return rc;
+  if ((rc = prefill(e))) return rc;
+  e->st.prefilled = true;
+  B200_CUDA_OK(cudaEventRecord(e->ev1, s));
+  const int B = e->st.B;
+  const bool record = logits_bf16 != nullptr;
+  const bool eager = record;             // per-step logits copies -> no graph
+  const size_t lrow = (size_t)e->Vl;     // logits of this rank's vocab shard
+  // tensor parallel: every rank records the logits of ITS vocabulary shard ([max_new_tokens][B][ceil(V / tp)] rows,
+  // the last rank's rows are shorter); the host concatenates the shards
+  std::vector<int64_t> cbuf(B);
+  auto after_step = [&](int step) -> int {
+    if (record)
+      B200_CUDA_OK(cudaMemcpyAsync(logits_bf16 + (size_t)step * B * lrow, e->logits, (size_t)B * lrow * 2, cudaMemcpyDeviceToHost, s));
+    if (cb) {
+      B200_CUDA_OK(cudaMemcpyAsync(e->h_out_tokens, e->d_out_tokens, (size_t)B * e->out_ld * 4, cudaMemcpyDeviceToHost, s));
+      B200_CUDA_OK(cudaMemcpyAsync(e->h_state, e->d_state, sizeof(StepState), cudaMemcpyDeviceToHost, s));
+      B200_CUDA_OK(cudaStreamSynchronize(s));
+      if (e->h_state->step > step) {
+        for (int b = 0; b < B; ++b) cbuf[b] = e->h_out_tokens[(size_t)b * e->out_ld + step];
+        if (cb(user, step, cbuf.data(), B)) return 1;
+      }
+      return e->h_state->done ? 2 : 0;
+    }
+    return 0;
+  };
+  int steps = 0;
+  int ar = after_step(0);
+  // Tensor parallel: only the leader has a callback, so a `done` seen after the first token (EOS first / a stop sequence
+  // that matches token 0) must not make it skip decode steps the followers still run — their all-reduces would wait for
+  // it forever.  Every rank leaves at the shared i % 8 poll below; a user abort (ar == 1) is honoured there as well.
+  bool aborted = ar == 1;
+  if (e->cfg.tp_size > 1) ar = 0;
+  if (ar == 0) {
+    for (int i = 1; i < max_new; ++i) {
+      if ((rc = decode_step(e, !eager))) return rc;
+      ++steps;
+      ar = after_step(i);
+      // under TP every rank must leave the loop at the same step (the next step contains collectives), so the
+      // only exit points are the shared polling cadence below; a streaming leader just stops receiving tokens.
+      if (ar && e->cfg.tp_size == 1) break;
+      if (ar == 1) aborted = true;
+      if (ar && e->cfg.tp_size > 1) ar = 0;
+      if ((!cb || e->cfg.tp_size > 1) && (i % 8) == 0) {  // poll the device-side done flag without a per-token sync
+        B200_CUDA_OK(cudaMemcpyAsync(e->h_state, e->d_state, sizeof(StepState), cudaMemcpyDeviceToHost, s));
+        B200_CUDA_OK(cudaStreamSynchronize(s));
+        if (e->h_state->done) break;
+      }
+    }
+  }
+  B200_CUDA_OK(cudaEventRecord(e->ev2, s));
+  if ((rc = fetch_result(e, out_ids, out_len, stop_triggered))) return rc;
+  B200_CUDA_OK(cudaEventElapsedTime(&e->timing.prefill_ms, e->ev0, e->ev1));
+  B200_CUDA_OK(cudaEventElapsedTime(&e->timing.decode_ms, e->ev1, e->ev2));
+  e->timing.decode_steps = steps;
+  e->timing.kernel_launches = e->launches;
+  return (ar == 1 || aborted) ? 1 : 0;
+}
 
 // ---- continuous batching ---------------------------------------------------------------------------
 static int cb_alloc(b200_engine* e) {
@@ -1115,48 +1213,29 @@ static int cb_take_page(b200_engine* e) {
 static int cb_prefill_pending(b200_engine* e, long long budget) {
   if (e->cb_pending.empty()) return 0;
   budget = std::min<long long>(budget, e->cap_T);
-  struct Part { size_t idx; int start, count; bool fin; };
-  std::vector<Part> parts;
+  // the pass takes a prefix of the FIFO: row i is cb_pending[i]
+  std::vector<PrefillRow<int32_t>> parts;
   long long left = budget;
   for (size_t i = 0; i < e->cb_pending.size() && (int)parts.size() < e->rows_cap; ++i) {
     const auto& pd = e->cb_pending[i];
     const int rem = (int)pd.toks.size() - pd.done;
     int c = rem <= left ? rem : (int)((left / 128) * 128);
     if (c <= 0) break;
-    parts.push_back(Part{i, pd.done, c, c == rem});
+    parts.push_back({pd.slot, pd.toks.data() + pd.done, pd.done, c, c == rem});
     left -= c;
     if (c < rem) break;       // budget exhausted inside this prompt: FIFO, later prompts wait
   }
   if (parts.empty()) return 0;
   const int n = (int)parts.size();
   int T = 0, max_len = 0, nfin = 0;
-  for (auto& pt : parts) { T += pt.count; max_len = std::max(max_len, pt.count); nfin += pt.fin ? 1 : 0; }
-  cudaStream_t s = e->stream;
-  int32_t* flat = e->h_stage;   // tok | tok_seq | tok_pos | cu | seq_slot | kv_off | last_rows | fin_slot
-  B200_REQUIRE((size_t)(3 * T + 5 * n + 1) <= e->h_stage_elems, "prompt staging buffer too small");
-  int32_t *h_tok = flat, *h_seq = flat + T, *h_pos = flat + 2 * T, *h_cu = flat + 3 * T, *h_slot = h_cu + n + 1, *h_off = h_slot + n,
-          *h_last = h_off + n, *h_fin = h_last + n;
-  int t = 0, f = 0;
   std::vector<int> lens(n);
   for (int i = 0; i < n; ++i) {
-    const auto& pd = e->cb_pending[parts[i].idx];
-    h_cu[i] = t;
-    for (int k = 0; k < parts[i].count; ++k, ++t) { h_tok[t] = pd.toks[parts[i].start + k]; h_seq[t] = pd.slot; h_pos[t] = parts[i].start + k; }
-    h_slot[i] = pd.slot; h_off[i] = parts[i].start; lens[i] = parts[i].count;
-    if (parts[i].fin) { h_last[f] = t - 1; h_fin[f] = pd.slot; ++f; }
+    T += parts[i].count; max_len = std::max(max_len, parts[i].count); nfin += parts[i].last ? 1 : 0; lens[i] = parts[i].count;
   }
-  h_cu[n] = t;
-  B200_CUDA_OK(cudaMemcpyAsync(e->d_tok, h_tok, (size_t)T * 4, cudaMemcpyHostToDevice, s));
-  B200_CUDA_OK(cudaMemcpyAsync(e->d_tok_seq, h_seq, (size_t)T * 4, cudaMemcpyHostToDevice, s));
-  B200_CUDA_OK(cudaMemcpyAsync(e->d_tok_pos, h_pos, (size_t)T * 4, cudaMemcpyHostToDevice, s));
-  B200_CUDA_OK(cudaMemcpyAsync(e->d_cu, h_cu, (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, s));
-  B200_CUDA_OK(cudaMemcpyAsync(e->d_seq_slot, h_slot, (size_t)n * 4, cudaMemcpyHostToDevice, s));
-  B200_CUDA_OK(cudaMemcpyAsync(e->d_kv_off, h_off, (size_t)n * 4, cudaMemcpyHostToDevice, s));
-  if (nfin) {
-    B200_CUDA_OK(cudaMemcpyAsync(e->d_last_rows, h_last, (size_t)nfin * 4, cudaMemcpyHostToDevice, s));
-    B200_CUDA_OK(cudaMemcpyAsync(e->d_cb_rec, h_fin, (size_t)nfin * 4, cudaMemcpyHostToDevice, s));   // row -> slot of the finishing rows
-  }
+  cudaStream_t s = e->stream;
   int rc;
+  // d_cb_rec: row -> slot of the finishing rows
+  if ((rc = pack_prefill(e, parts, e->d_kv_off, e->d_cb_rec))) return rc;
   if ((rc = prefill_layers(e, PrefillPass{T, n, max_len, lens.data(), e->d_kv_off}))) return rc;
   if (nfin) {
     B200_CUDA_OK(launch_k(gather_rows_kernel, dim3(nfin), dim3(128), 0, s, (const bf16*)e->xn, (const int32_t*)e->d_last_rows, e->xl, e->H));
@@ -1167,9 +1246,9 @@ static int cb_prefill_pending(b200_engine* e, long long budget) {
   e->cb_stat[2] += T; e->cb_stat[4]++;
   // bookkeeping (front to back so that erasing does not disturb the indices still to be visited)
   for (int i = n - 1; i >= 0; --i) {
-    auto& pd = e->cb_pending[parts[i].idx];
+    auto& pd = e->cb_pending[i];
     pd.done += parts[i].count;
-    if (!parts[i].fin) continue;
+    if (!parts[i].last) continue;
     if (e->cb_prefix_on) {   // every full 128-token block of the prompt can now be shared with later requests
       const auto& pages = e->cb_slot_pages[pd.slot];
       unsigned long long parent = 0;
@@ -1186,7 +1265,7 @@ static int cb_prefill_pending(b200_engine* e, long long budget) {
     }
     e->cb_active.push_back(pd.slot);
     e->cb_rows_dirty = true;
-    e->cb_pending.erase(e->cb_pending.begin() + parts[i].idx);
+    e->cb_pending.erase(e->cb_pending.begin() + i);
   }
   return 0;
 }
@@ -1541,31 +1620,22 @@ int b200_engine_create(const b200_model_config_t* c, const void* nccl_id, b200_e
   if ((rc = dmalloc(e, &e->d_cu, 80))) return rc;
   if ((rc = dmalloc(e, &e->d_seq_slot, 80))) return rc;
   if ((rc = dmalloc(e, &e->d_last_rows, 80))) return rc;
-  if ((rc = dmalloc(e, &e->d_cur_len, 80))) return rc;
   if ((rc = dmalloc(e, &e->d_next_tok, 80))) return rc;
-  if ((rc = dmalloc(e, &e->d_dec_pos, 80))) return rc;
-  if ((rc = dmalloc(e, &e->d_finished, 80))) return rc;
+  // one block, so that restoring a staged batch's rows is one copy; the captured decode graphs hold these addresses
+  if ((rc = dmalloc(e, &e->d_cur_len, (size_t)6 * kMaxRows))) return rc;
+  e->d_dec_pos = e->d_cur_len + kMaxRows;
+  e->d_finished = e->d_cur_len + 2 * kMaxRows;
+  e->d_row_init = e->d_cur_len + 3 * kMaxRows;
   if ((rc = dmalloc(e, &e->d_out_tokens, (size_t)c->max_batch * e->out_ld))) return rc;
   if ((rc = dmalloc(e, &e->d_forced, (size_t)c->max_batch * e->out_ld))) return rc;
   if ((rc = dmalloc(e, &e->d_eos, 16))) return rc;
   if ((rc = dmalloc(e, &e->d_stop_tok, 1024))) return rc;
   if ((rc = dmalloc(e, &e->d_stop_off, 32))) return rc;
   if ((rc = dmalloc(e, &e->d_state, 1))) return rc;
-  e->h_stage_elems = 3 * T + 8 * 80;
+  e->h_stage_elems = 3 * T + 5 * kMaxRows + 1 + 3 * kMaxRows;
   if ((rc = hmalloc(e, &e->h_stage, e->h_stage_elems))) return rc;
   if ((rc = hmalloc(e, &e->h_state, 1))) return rc;
   if ((rc = hmalloc(e, &e->h_out_tokens, (size_t)c->max_batch * e->out_ld))) return rc;
-  {
-    const size_t raw = (size_t)c->max_batch * c->max_seq_len;
-    if ((rc = dmalloc(e, &e->d_raw_ids, raw))) return rc;
-    if ((rc = dmalloc(e, &e->d_raw_mask, raw))) return rc;
-    if ((rc = dmalloc(e, &e->d_pred, raw))) return rc;
-    if ((rc = dmalloc(e, &e->d_flat, T))) return rc;
-    if ((rc = dmalloc(e, &e->d_offs, 80))) return rc;
-    const size_t hraw = std::max(2 * raw, (T + 80) / 2 + 1);
-    if ((rc = hmalloc(e, &e->h_raw, hraw))) return rc;
-    if ((rc = hmalloc(e, &e->h_pred, raw))) return rc;
-  }
   if (tp > 1) {
     B200_REQUIRE(tp <= kMaxTp && kMaxRows <= kArRows, "tp_size exceeds the peer-exchange layout");
     const ArLayout lay = ArLayout::make(e->H);
@@ -1810,13 +1880,11 @@ int b200_run_staged(b200_engine_t* e, int32_t do_prefill, int32_t decode_steps) 
   B200_CUDA_OK(cudaSetDevice(e->cfg.device));
   int rc;
   if (do_prefill) {
-    // reset the per-request device state so the same staged prompt can be replayed: the raw rows are still
-    // resident on the device, so this re-runs the device-side concat and nothing crosses PCIe
+    // reset the per-request device state so the same staged prompt can be replayed: the packed prompt is still on
+    // the device (static prefill and decode only read it), so only the per-sequence rows and the step state are reset
     auto& st = e->st;
-    if (st.S > 0) pack_padded_kernel<<<1, 1024, 0, e->stream>>>(e->d_raw_ids, e->staged_mask ? e->d_raw_mask : nullptr, st.B, st.S, pack_out(e));
-    else pack_ragged_kernel<<<1, 1024, 0, e->stream>>>(e->d_flat, e->d_offs, st.B, pack_out(e));
-    B200_CUDA_OK(cudaGetLastError());
-    e->launches++;
+    B200_REQUIRE(st.B > 0, "run_staged: no staged prompt (continuous batching discards it)");
+    if ((rc = restore_rows(e))) return rc;
     StepState init{0, 0, 0, st.max_new};
     *e->h_state = init;
     B200_CUDA_OK(cudaMemcpyAsync(e->d_state, e->h_state, sizeof(StepState), cudaMemcpyHostToDevice, e->stream));
@@ -1858,115 +1926,21 @@ int b200_generate(b200_engine_t* e, const int64_t* ids, const int64_t* mask, int
                   uint16_t* logits_bf16, b200_token_callback cb, void* user) {
   B200_REQUIRE(e && ids && gp && out_ids && out_len, "null argument");
   B200_CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t s = e->stream;
-  e->launches = 0;
-  B200_CUDA_OK(cudaEventRecord(e->ev0, s));
-  int rc = stage_prompt(e, ids, mask, B, S, gp);
-  if (rc) return rc;
-  if ((rc = prefill(e))) return rc;
-  e->st.prefilled = true;
-  B200_CUDA_OK(cudaEventRecord(e->ev1, s));
-  const bool record = logits_bf16 != nullptr;
-  const bool eager = record;             // per-step logits copies -> no graph
-  const size_t lrow = (size_t)e->Vl;     // logits of this rank's vocab shard
-  // tensor parallel: every rank records the logits of ITS vocabulary shard ([max_new_tokens][B][ceil(V / tp)] rows,
-  // the last rank's rows are shorter); the host concatenates the shards
-  std::vector<int64_t> cbuf(B);
-  auto after_step = [&](int step) -> int {
-    if (record)
-      B200_CUDA_OK(cudaMemcpyAsync(logits_bf16 + (size_t)step * B * lrow, e->logits, (size_t)B * lrow * 2, cudaMemcpyDeviceToHost, s));
-    if (cb) {
-      B200_CUDA_OK(cudaMemcpyAsync(e->h_out_tokens, e->d_out_tokens, (size_t)B * e->out_ld * 4, cudaMemcpyDeviceToHost, s));
-      B200_CUDA_OK(cudaMemcpyAsync(e->h_state, e->d_state, sizeof(StepState), cudaMemcpyDeviceToHost, s));
-      B200_CUDA_OK(cudaStreamSynchronize(s));
-      if (e->h_state->step > step) {
-        for (int b = 0; b < B; ++b) cbuf[b] = e->h_out_tokens[(size_t)b * e->out_ld + step];
-        if (cb(user, step, cbuf.data(), B)) return 1;
-      }
-      return e->h_state->done ? 2 : 0;
-    }
-    return 0;
-  };
-  int steps = 0;
-  int ar = after_step(0);
-  // Tensor parallel: only the leader has a callback, so a `done` seen after the first token (EOS first / a stop sequence
-  // that matches token 0) must not make it skip decode steps the followers still run — their all-reduces would wait for
-  // it forever.  Every rank leaves at the shared i % 8 poll below; a user abort (ar == 1) is honoured there as well.
-  bool aborted = ar == 1;
-  if (e->cfg.tp_size > 1) ar = 0;
-  if (ar == 0) {
-    for (int i = 1; i < gp->max_new_tokens; ++i) {
-      if ((rc = decode_step(e, !eager))) return rc;
-      ++steps;
-      ar = after_step(i);
-      // under TP every rank must leave the loop at the same step (the next step contains collectives), so the
-      // only exit points are the shared polling cadence below; a streaming leader just stops receiving tokens.
-      if (ar && e->cfg.tp_size == 1) break;
-      if (ar == 1) aborted = true;
-      if (ar && e->cfg.tp_size > 1) ar = 0;
-      if ((!cb || e->cfg.tp_size > 1) && (i % 8) == 0) {  // poll the device-side done flag without a per-token sync
-        B200_CUDA_OK(cudaMemcpyAsync(e->h_state, e->d_state, sizeof(StepState), cudaMemcpyDeviceToHost, s));
-        B200_CUDA_OK(cudaStreamSynchronize(s));
-        if (e->h_state->done) break;
-      }
-    }
-  }
-  B200_CUDA_OK(cudaEventRecord(e->ev2, s));
-  if ((rc = fetch_result(e, out_ids, out_len, stop_triggered))) return rc;
-  B200_CUDA_OK(cudaEventElapsedTime(&e->timing.prefill_ms, e->ev0, e->ev1));
-  B200_CUDA_OK(cudaEventElapsedTime(&e->timing.decode_ms, e->ev1, e->ev2));
-  e->timing.decode_steps = steps;
-  e->timing.kernel_launches = e->launches;
-  return (ar == 1 || aborted) ? 1 : 0;
+  return generate(e, [&] { return stage_prompt(e, ids, mask, B, S, gp); }, gp->max_new_tokens, logits_bf16, cb, user,
+                  out_ids, out_len, stop_triggered);
 }
 
 // Replaces the body of BatchHandler.batchPredict (pkg/batcher/handler.go:99-155): the instances of every
-// waiting request (ragged token rows) are concatenated ON DEVICE, generated in one batch, and the predictions
-// come back as one [n_rows][max_new_tokens] matrix in instance order, so each request's answer is the
-// contiguous slice [first, first+count) the batcher recorded (handler.go:139-150).
+// waiting request (ragged token rows) are generated in one batch, and the predictions come back as one
+// [n_rows][max_new_tokens] matrix in instance order, so each request's answer is the contiguous slice
+// [first, first+count) the batcher recorded (handler.go:139-150).
 int b200_batch_predict(b200_engine_t* e, const int64_t* const* rows, const int32_t* row_lens, int32_t n_rows,
                        const b200_gen_params_t* gp, int64_t* predictions, int32_t* n_generated,
                        int32_t* stop_triggered) {
   B200_REQUIRE(e && rows && row_lens && gp && predictions && n_generated, "null argument");
   B200_CUDA_OK(cudaSetDevice(e->cfg.device));
-  cudaStream_t s = e->stream;
-  e->launches = 0;
-  B200_CUDA_OK(cudaEventRecord(e->ev0, s));
-  int rc = stage_ragged(e, rows, row_lens, n_rows, gp);
-  if (rc) return rc;
-  if ((rc = prefill(e))) return rc;
-  e->st.prefilled = true;
-  B200_CUDA_OK(cudaEventRecord(e->ev1, s));
-  int steps = 0;
-  for (int i = 1; i < gp->max_new_tokens; ++i) {
-    if ((rc = decode_step(e, true))) return rc;
-    ++steps;
-    if ((i % 8) == 0) {
-      B200_CUDA_OK(cudaMemcpyAsync(e->h_state, e->d_state, sizeof(StepState), cudaMemcpyDeviceToHost, s));
-      B200_CUDA_OK(cudaStreamSynchronize(s));
-      if (e->h_state->done) break;
-    }
-  }
-  B200_CUDA_OK(cudaEventRecord(e->ev2, s));
-  B200_CUDA_OK(cudaMemcpyAsync(e->h_state, e->d_state, sizeof(StepState), cudaMemcpyDeviceToHost, s));
-  B200_CUDA_OK(cudaStreamSynchronize(s));
-  { int frc = check_fault(e); if (frc) return frc; }
-  const int T = e->h_state->step;
-  scatter_predictions_kernel<<<n_rows, 128, 0, s>>>(e->d_out_tokens, e->out_ld, n_rows, T, e->d_pred);
-  B200_CUDA_OK(cudaGetLastError());
-  e->launches++;
-  B200_CUDA_OK(cudaMemcpyAsync(e->h_pred, e->d_pred, (size_t)n_rows * T * 8, cudaMemcpyDeviceToHost, s));
-  B200_CUDA_OK(cudaStreamSynchronize(s));
-  for (int b = 0; b < n_rows; ++b)
-    for (int i = 0; i < gp->max_new_tokens; ++i)
-      predictions[(size_t)b * gp->max_new_tokens + i] = i < T ? e->h_pred[(size_t)b * T + i] : gp->pad_token_id;
-  *n_generated = T;
-  if (stop_triggered) *stop_triggered = e->h_state->stop_triggered;
-  B200_CUDA_OK(cudaEventElapsedTime(&e->timing.prefill_ms, e->ev0, e->ev1));
-  B200_CUDA_OK(cudaEventElapsedTime(&e->timing.decode_ms, e->ev1, e->ev2));
-  e->timing.decode_steps = steps;
-  e->timing.kernel_launches = e->launches;
-  return 0;
+  return generate(e, [&] { return stage_ragged(e, rows, row_lens, n_rows, gp); }, gp->max_new_tokens, nullptr, nullptr,
+                  nullptr, predictions, n_generated, stop_triggered);
 }
 
 // ---- batcher trigger state machine (pkg/batcher/handler.go:157-199) ---------------------------------
@@ -2092,6 +2066,7 @@ int b200_cb_begin(b200_engine_t* e, int64_t pad_token_id, const int64_t* eos_tok
   e->cb_active.clear();
   e->cb_rows_dirty = true;
   e->cb_on = true;
+  e->st = b200_engine::Staged{};   // the batcher overwrites the packed prompt and the page table of a staged batch
   return 0;
 }
 

@@ -247,7 +247,7 @@ class B200Engine:
     # ------------------------------------------------------------------ batcher leg (ragged rows, no padding)
     def batch_predict(self, rows: Sequence[Sequence[int]], *, max_new_tokens: int, pad_token_id: Optional[int] = 0,
                       eos_token_ids: Sequence[int] = (), stop_sequences: Sequence[Sequence[int]] = ()):
-        """-> (predictions int64 [n_rows, T], stop_triggered). Rows are concatenated on the device."""
+        """-> (predictions int64 [n_rows, T], stop_triggered). The rows run as one batch, without padding."""
         n = len(rows)
         arrs = [(C.c_int64 * len(r))(*[int(t) for t in r]) for r in rows]
         ptrs = (C.c_void_p * n)(*[C.cast(a, C.c_void_p) for a in arrs])

@@ -675,7 +675,7 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
                 raise InvalidInput("attention_mask must be left padding (zeros, then ones) with at least one token per row")
         if not isinstance(payload, InferRequest) and not as_text and self._cb is None:
             # the V1 `:predict` leg the batcher fronts: the instances (ragged token rows, one per instance of every merged
-            # request) are concatenated on the device and the predictions come back as one matrix in instance order —
+            # request) run as one batch and the predictions come back as one matrix in instance order —
             # the body of BatchHandler.batchPredict (pkg/batcher/handler.go:99-155) as one C-ABI call
             rows = self._unpadded_rows(ids, mask)
             pred, _ = await self._submit(lambda: self._batch_predict(rows, max_new_tokens=max_tokens, pad_token_id=self._pad_token_id,

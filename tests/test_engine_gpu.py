@@ -305,6 +305,27 @@ def test_kv_host_offload_tier_roundtrip(engines):
     assert torch.equal(eng.fetch_staged(), ref)
 
 
+@pytest.mark.parametrize("name,use_mask", [("tiny_g2_ids", False), ("tiny_g2_text", True)])   # plain / left-padded rows
+def test_staged_prompt_replays_like_generate(engines, name, use_mask):
+    """b200_run_staged(do_prefill=1) replays the staged prompt from what staging left on the device, as bench.py times
+    it: every replay gives generate's ids.  Continuous batching overwrites the packed prompt and the page table, so a
+    replay after a continuous-batching session is refused."""
+    from kserve_b200._lib import B200Error
+    c = load_case(name)
+    eng = engines(c)
+    pad, T = c["meta"]["pad_token_id"], c["T"]
+    mask = c["mask"] if use_mask else None
+    ref = eng.generate(c["input_ids"], mask, max_new_tokens=T, pad_token_id=pad).output_ids
+    eng.stage(c["input_ids"], mask, max_new_tokens=T, pad_token_id=pad)
+    for _ in range(3):
+        eng.run_staged(True, T - 1)
+        assert torch.equal(eng.fetch_staged(), ref)
+    eng.cb_begin(pad)
+    eng.cb_end()
+    with pytest.raises(B200Error, match="no staged prompt"):
+        eng.run_staged(True, T - 1)
+
+
 def test_long_context_3968_prompt_tokens():
     """A 3968-token prompt (31 query tiles of 128) plus 64 generated tokens on tiny_g2_rope3, whose max_position of 4096
     bounds both: every step's logits against the oracle's forward (on the CPU) over the engine's own ids, at the stated

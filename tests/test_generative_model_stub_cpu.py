@@ -244,7 +244,7 @@ def test_continuous_batching_wiring_and_stream_disconnect(served):
 
 
 def test_enable_batcher_installs_batch_handler_in_front_of_predict(served):
-    """--enable_batcher: concurrent V1 :predict requests are merged into ONE engine call (device-side concat of their
+    """--enable_batcher: concurrent V1 :predict requests are merged into ONE engine call (over all their
     ragged instances) and each caller gets {"message", "batchId", "predictions"} with its own slice — the wiring of
     cmd/agent/main.go:431-433 + pkg/batcher/handler.go:222-266; scenario of test/e2e/batcher/test_batcher.py:33-85
     (same batchId for requests that were batched together)."""

@@ -151,10 +151,32 @@ def test_batch_predict_ragged_rows_equal_padded_generate(served):
     assert torch.equal(pred, ref.output_ids[:, c["S"]:]) and not stop
 
 
+@pytest.mark.parametrize("ends", ["eos", "stop"])
+def test_batch_predict_rows_ended_early_equal_padded_generate(served, ends):
+    """As above when an EOS id or a stop sequence ends rows before max_new_tokens: the unpadded rows through
+    b200_batch_predict give b200_generate's tokens on the left-padded batch, number of steps and stop flag included
+    (a row that is done is filled with the pad id)."""
+    client, model, tok, c = served
+    eng, S, T, pad = model._engine, c["S"], c["T"], 256
+    rows = [c["input_ids"][b][c["mask"][b].bool()].tolist() for b in range(c["input_ids"].shape[0])]
+    free = eng.generate(c["input_ids"], c["mask"], max_new_tokens=T, pad_token_id=pad).output_ids[:, S:]
+    kw = {"eos_token_ids": [int(free[1, 2])]} if ends == "eos" else {"stop_sequences": [free[0, 3:5].tolist()]}
+    pred, stop = eng.batch_predict(rows, max_new_tokens=T, pad_token_id=pad, **kw)
+    ref = eng.generate(c["input_ids"], c["mask"], max_new_tokens=T, pad_token_id=pad, **kw)
+    if ends == "eos":        # row 1 emits the EOS id by step 2, then pads
+        row = ref.output_ids[1, S:].tolist()
+        first = row.index(kw["eos_token_ids"][0])
+        assert first <= 2 and all(t == pad for t in row[first + 1:])
+    else:
+        assert ref.stop_triggered and ref.num_generated < T
+    assert pred.shape[1] == ref.num_generated and stop == ref.stop_triggered == (ends == "stop")
+    assert torch.equal(pred, ref.output_ids[:, S:])
+
+
 def test_enable_batcher_served_over_http(served):
     """--enable_batcher on the served path (VERDICT r01 #7): the batcher sits in front of /v1/models/{m}:predict
-    (cmd/agent/main.go:431-433), concurrent requests are merged and run as ONE b200_batch_predict call (device-side concat
-    of the ragged rows + scatter), every caller gets its own slice under a shared batchId
+    (cmd/agent/main.go:431-433), concurrent requests are merged and run as ONE b200_batch_predict call over
+    their ragged rows, every caller gets its own slice under a shared batchId
     (test/e2e/batcher/test_batcher.py:33-85)."""
     import concurrent.futures
     from kserve_b200.kserve_api import ModelServer

@@ -2,7 +2,7 @@
 closed-loop clients, one instance (one ragged token-id prompt, U[512,1024] tokens) per request.
 
 The Go sidecar cannot be built here (no Go toolchain): the same trigger state machine (C ABI b200_batcher_*) is
-driven by the Python BatchHandler; the downstream call is b200_batch_predict (device-side concat / scatter).
+driven by the Python BatchHandler; the downstream call is one b200_batch_predict per formed batch.
 Reports tokens/s, request latency and TTFT percentiles and the mean formed batch size."""
 import asyncio
 import json

@@ -4,7 +4,7 @@ FastAPI routes of kserve_b200.kserve_api) fronting Llama-3-8B dims (random init)
     MODE=continuous  POST /openai/v1/completions (token-id prompts) served by the iteration-level scheduler
                      (--continuous_batching, chunked prefill, up to SLOTS resident sequences)
     MODE=batcher     POST /v1/models/llama:predict behind --enable_batcher (maxBatchSize 64, maxLatency 50 ms): formed
-                     batches run as one b200_batch_predict call (device-side concat / scatter), like the Go agent + predictor
+                     batches run as one b200_batch_predict call, like the Go agent + predictor
 
 Every request carries one ragged prompt of U[512,1024] token ids and asks for 128 new tokens.  Latency is measured at the
 client (aiohttp); TTFT is taken where the first token becomes available to the server (scheduler: submit -> first token;
