@@ -74,8 +74,11 @@ int b200_engine_ipc_import(b200_engine_t* e, const void* handles, int32_t n);
  * `mlp.experts.gate_up_proj` [E,2I,H] and `mlp.experts.down_proj` [E,H,I].  Qwen2 checkpoints add the 1-D
  * projection biases `self_attn.q_proj.bias` [num_heads*128] and `self_attn.{k,v}_proj.bias` [num_kv_heads*128]; they are
  * sharded like the weights' rows and added in fp32 before the projection's one bf16 rounding (before RoPE).
- * b200_engine_finalize_weights fails if a tensor is missing: it takes 3 + 9 L tensors, or 3 + 12 L when every layer has
- * all three biases. */
+ * Qwen3 checkpoints add `self_attn.q_norm.weight` and `self_attn.k_norm.weight` [128]: one RMSNorm weight each, shared by
+ * every head and replicated on every rank, applied (eps = rms_eps) to each q and k head between the projection and RoPE.
+ * b200_engine_finalize_weights fails if a tensor is missing: it takes 3 + 9 L tensors, + 3 L when every layer has all
+ * three biases, or + 2 L when every layer has both q/k norm weights; a partial set, and biases together with q/k norms,
+ * are refused with the tensor named. */
 int b200_engine_set_weight(b200_engine_t* e, const char* hf_name, const void* data, int on_device,
                            int ndim, const int64_t* shape);
 /* weight_format 1: the seven projection weights `model.layers.N.{self_attn.{q,k,v,o}_proj, mlp.{gate,up,down}_proj}.weight`
@@ -246,9 +249,32 @@ int b200_op_attn_decode_fused_kv8(const void* qkv, int64_t ld_qkv, const float* 
                                   const int32_t* page_table, int max_pages, const int32_t* seq_slot, const int32_t* tok_pos,
                                   int B, int nh, int nkv, int splits, float* part_o, float* part_ml, int32_t* split_counter,
                                   void* stream);
+/* b200_op_attn_decode_fused with Qwen3's per-head q / k RMSNorm (q_norm_w, k_norm_w: bf16 [128], both or NULL; eps) on the
+ * bf16-rounded projection row before RoPE, for a bf16 (kv8 0) or float8_e4m3fn (kv8 1) cache */
+int b200_op_attn_decode_fused_norm(const void* qkv, int64_t ld_qkv, const float* qkv_partial, int qkv_splits,
+                                   int64_t split_stride, int64_t ld_partial, const void* qkv_bias, const void* q_norm_w,
+                                   const void* k_norm_w, float eps, const void* cos_tab, const void* sin_tab, void* out,
+                                   int64_t ldo, void* kcache, void* vcache, int kv8, const int32_t* page_table, int max_pages,
+                                   const int32_t* seq_slot, const int32_t* tok_pos, int B, int nh, int nkv, int splits,
+                                   float* part_o, float* part_ml, int32_t* split_counter, void* stream);
 int b200_op_rope_kv(const void* qkv, int64_t ld, void* q_out, int64_t ldq, void* kcache, void* vcache,
                     const int32_t* page_table, int max_pages, const int32_t* tok_seq, const int32_t* tok_pos,
                     const void* cos_tab, const void* sin_tab, int T, int nh, int nkv, void* stream);
+/* b200_op_rope_kv with Qwen3's per-head q / k RMSNorm before RoPE (q_norm_w, k_norm_w: bf16 [128], both or NULL) and a
+ * bf16 (kv8 0) or float8_e4m3fn (kv8 1) cache; one token per CTA, as the engine's B200_NO_ROPE_FUSION=1 path launches it */
+int b200_op_rope_kv_norm(const void* qkv, int64_t ld, void* q_out, int64_t ldq, void* kcache, void* vcache, int kv8,
+                         const int32_t* page_table, int max_pages, const int32_t* tok_seq, const int32_t* tok_pos,
+                         const void* cos_tab, const void* sin_tab, const void* q_norm_w, const void* k_norm_w, float eps,
+                         int T, int nh, int nkv, void* stream);
+/* The prefill QKV projection as the engine launches it: x bf16 [T][H] times wqkv bf16 [(nh + 2 nkv) * 128][H] (q | k | v
+ * heads), with an optional bias [(nh + 2 nkv) * 128] added before the one bf16 rounding, optional Qwen3 q / k norms
+ * (q_norm_w, k_norm_w: bf16 [128], both or NULL; not with a bias), then RoPE at tok_pos, all in the GEMM's epilogue
+ * (EPI_ROPE_KV).  The roped q heads go to out[t][0 : nh * 128] (ldo >= (nh + 2 nkv) * 128; the other columns are not
+ * written); k and v go to the paged caches, bf16 (kv8 0) or float8_e4m3fn codes (kv8 1), like b200_op_rope_kv. */
+int b200_op_qkv_rope_kv(const void* x, const void* wqkv, void* out, int64_t ldo, int T, int H, int nh, int nkv,
+                        const void* bias, const void* q_norm_w, const void* k_norm_w, float eps, void* kcache, void* vcache,
+                        int kv8, const int32_t* page_table, int max_pages, const int32_t* tok_seq, const int32_t* tok_pos,
+                        const void* cos_tab, const void* sin_tab, void* stream);
 int b200_op_argmax(const void* logits, int64_t ld, int B, int V, float* out_val, int32_t* out_idx, void* stream);
 /* The logits processors and the draw of one decode step, launched exactly as the engine launches them (one CTA of 1024
  * threads per row).  logits bf16 [B][ld] (ld >= V); params are mapped as b200_generate / b200_cb_admit map them.

@@ -84,6 +84,13 @@ def load() -> C.CDLL:
                                               C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
     lib.b200_op_rope_kv.argtypes = [vp, i64, vp, i64, vp, vp, vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int,
                                     C.c_int, vp]
+    lib.b200_op_attn_decode_fused_norm.argtypes = [vp, i64, vp, C.c_int, i64, i64, vp, vp, vp, C.c_float, vp, vp, vp, i64, vp, vp,
+                                                   C.c_int, vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp,
+                                                   vp, vp]
+    lib.b200_op_rope_kv_norm.argtypes = [vp, i64, vp, i64, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, C.c_float,
+                                         C.c_int, C.c_int, C.c_int, vp]
+    lib.b200_op_qkv_rope_kv.argtypes = [vp, vp, vp, i64, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_float, vp, vp,
+                                        C.c_int, vp, C.c_int, vp, vp, vp, vp, vp]
     lib.b200_op_argmax.argtypes = [vp, i64, C.c_int, C.c_int, vp, vp, vp]
     lib.b200_op_sample.argtypes = [vp, i64, C.c_int, C.c_int, vp, vp, vp, C.c_int, C.POINTER(GenParams), i32, vp, vp, vp]
     lib.b200_op_moe_block.argtypes = [C.c_int, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,

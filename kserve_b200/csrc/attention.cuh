@@ -239,6 +239,9 @@ struct AttnDecodeParams {
   const bf16* qkv_bias;   // [ld_qkv] projection bias added to the summed partials before their bf16 rounding (nullptr = none;
                           // a bf16 `qkv` row already carries it from the GEMM epilogue)
   const bf16* cos_tab; const bf16* sin_tab;
+  // Qwen3: per-head RMSNorm of the G q heads (q_norm_w) and the k head (k_norm_w), [128] each, on the bf16-rounded row
+  // before RoPE, in common.cuh's qknorm order (so the appended k equals rope_kv_kernel's); both nullptr = none
+  const bf16* q_norm_w; const bf16* k_norm_w; float qk_eps;
   bf16* kcache_w; bf16* vcache_w;       // (e4m3 codes in attn_decode_kernel<true>, which appends e4m3(k), e4m3(v))
   // splits > 1: per-(sequence, kv head) arrival counters (zero between launches).  When set, the LAST split CTA to
   // arrive merges the partials itself (in split order: deterministic) and no attn_combine_kernel follows — one kernel
@@ -359,6 +362,29 @@ __global__ void __launch_bounds__(kAttnThreads) attn_decode_kernel(const AttnDec
       for (int i = 0; i < 8; ++i) s_raw[hl * kHeadDim + c + i] = f[i];
     }
     __syncthreads();
+    if (p.q_norm_w) {
+      // thread (head hl, part qd) sums the squares of dims 8j + 2qd + {0, 1} and rewrites exactly those dims, so no
+      // barrier is needed between the sums and the writes; (G + 1) * 4 <= 36 threads, the quads complete
+      const int gi = threadIdx.x;
+      const unsigned act = __ballot_sync(0xffffffffu, gi < (G + 1) * 4);
+      if (gi < (G + 1) * 4) {
+        const int hl = gi >> 2, qd = gi & 3;
+        float* row = s_raw + hl * kHeadDim + 2 * qd;
+        float sh = 0.f;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) sh = qknorm_acc(sh, row[8 * j], row[8 * j + 1]);
+        sh += __shfl_xor_sync(act, sh, 1);
+        sh += __shfl_xor_sync(act, sh, 2);
+        const float r = qknorm_rstd(sh, p.qk_eps);
+        const bf16* w = (hl < G ? p.q_norm_w : p.k_norm_w) + 2 * qd;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          row[8 * j] = qknorm_apply(row[8 * j], r, __bfloat162float(w[8 * j]));
+          row[8 * j + 1] = qknorm_apply(row[8 * j + 1], r, __bfloat162float(w[8 * j + 1]));
+        }
+      }
+      __syncthreads();
+    }
     const int items = (G + 1) * 8 + 16;   // roped heads (q heads + k) x 8 threads, then 16 threads copy v
     for (int it = threadIdx.x; it < items; it += kAttnThreads) {
       if (it < (G + 1) * 8) {

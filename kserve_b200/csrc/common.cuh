@@ -56,6 +56,18 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
   return __bfloat1622float2(v);
 }
 
+// Per-head RMSNorm of q and k (Qwen3RMSNorm over one head's 128 dims, between the projection and RoPE).  The prefill
+// QKV epilogue, rope_kv_kernel and the decode attention prologue all normalise with these helpers, in this one order of
+// the 128 squares, so they produce the same bits from the same bf16 inputs.  The order is the one the wgmma fragment
+// gives for free: part qd (0..3) accumulates dims 8j + 2qd and 8j + 2qd + 1 for j = 0..15 in increasing j (the dims quad
+// lane qd holds), and the head's sum is (S0 + S1) + (S2 + S3), which two shfl_xor steps (1, then 2) produce in every lane.
+__device__ __forceinline__ float qknorm_acc(float s, float a0, float a1) { return fmaf(a1, a1, fmaf(a0, a0, s)); }
+__device__ __forceinline__ float qknorm_sum(float s0, float s1, float s2, float s3) { return (s0 + s1) + (s2 + s3); }
+// 1 / sqrt(mean of the squares + eps)
+__device__ __forceinline__ float qknorm_rstd(float sumsq, float eps) { return rsqrtf(sumsq * (1.0f / 128.0f) + eps); }
+// bf16(bf16(a * r) * w): Qwen3RMSNorm casts to the input dtype before the weight multiply
+__device__ __forceinline__ float qknorm_apply(float a, float r, float w) { return bf16_round(bf16_round(a * r) * w); }
+
 // FP8 KV cache codes: e4m3(clamp(x, -448, 448)), round to nearest even; NaN stays NaN.  `lo` goes to the lower byte.
 __device__ __forceinline__ uint32_t e4m3x2_rn_sat(float lo, float hi) {
   uint16_t r;

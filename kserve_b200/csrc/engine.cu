@@ -72,6 +72,7 @@ struct LayerW {
   bf16 *wqkv = nullptr, *wo = nullptr, *wgu = nullptr, *wdown = nullptr, *ln1 = nullptr, *ln2 = nullptr;
   bf16 *wr = nullptr, *wgu_e = nullptr, *wdown_e = nullptr;   // MoE: router [E][H], experts [E][2I][H] / [E][H][I]
   bf16* bqkv = nullptr;   // q/k/v projection bias [qkv_cols] in wqkv's [q | k | v] order (Qwen2); nullptr = none
+  bf16* qk_norm = nullptr;   // per-head q / k RMSNorm weights [2][128], q_norm then k_norm (Qwen3); nullptr = none
   // weight_format 1: the four projections as e4m3 codes in the bf16 matrices' layouts (the bf16 pointers above stay null)
   // and the bf16 scale of every fused row (o / down: all H rows on every rank)
   uint8_t *wqkv8 = nullptr, *wo8 = nullptr, *wgu8 = nullptr, *wdown8 = nullptr;
@@ -517,6 +518,7 @@ static int decode_layers(b200_engine* e, int B) {
       ap.qkv_partial = e->ws; ap.qkv_splits = sp; ap.qkv_split_stride = (long long)B * e->qkv_cols; ap.ld_qkv_partial = e->qkv_cols;
       ap.qkv_bias = w.bqkv;
     }
+    if (w.qk_norm) { ap.q_norm_w = w.qk_norm; ap.k_norm_w = w.qk_norm + kHeadDim; ap.qk_eps = e->cfg.rms_eps; }
     static const bool fold = getenv("B200_ATTN_COMBINE_KERNEL") == nullptr;   // =1: separate attn_combine_kernel (A/B)
     ap.split_counter = fold ? e->attn_split_cnt : nullptr;
     if ((rc = launch_attn_decode(ap, B, s, e->kv8))) return rc;
@@ -649,6 +651,7 @@ static int prefill_layers(b200_engine* e, const PrefillPass& pp) {
     rp.tok_seq = e->d_tok_seq + r0; rp.tok_pos = e->d_tok_pos + r0;
     rp.kcache = kc; rp.vcache = vc; rp.page_table = e->d_page_table; rp.max_pages = e->max_pages;
     rp.cos_tab = e->cos_tab; rp.sin_tab = e->sin_tab; rp.nh = e->nh; rp.nkv = e->nkv; rp.kv8 = e->kv8;
+    if (w.qk_norm) { rp.q_norm_w = w.qk_norm; rp.k_norm_w = w.qk_norm + kHeadDim; rp.qk_eps = e->cfg.rms_eps; }
     // RoPE + KV append in the QKV GEMM's epilogue (the separate rope_kv_kernel pass re-read and re-wrote 750 MB per layer
     // at 0.37 of the HBM peak); B200_NO_ROPE_FUSION=1 restores the two-kernel path
     static const bool rope_fused = getenv("B200_NO_ROPE_FUSION") == nullptr;
@@ -1739,6 +1742,11 @@ int b200_engine_set_weight(b200_engine_t* e, const char* name, const void* data,
       B200_REQUIRE(expect(full, -1), "shape mismatch for " + n);
       if (!w.bqkv && (rc = dmalloc(e, &w.bqkv, (size_t)e->qkv_cols))) return rc;
       rc = copy_rows(w.bqkv + off, src, r * len, len, 1, dev);
+    } else if (rest == "self_attn.q_norm.weight" || rest == "self_attn.k_norm.weight") {
+      // Qwen3: one [head_dim] weight each, shared by every head and replicated on every tensor-parallel rank
+      B200_REQUIRE(expect(kHeadDim, -1), "shape mismatch for " + n);
+      if (!w.qk_norm && (rc = dmalloc(e, &w.qk_norm, (size_t)2 * kHeadDim))) return rc;
+      rc = copy_rows(w.qk_norm + (rest[10] == 'k' ? kHeadDim : 0), src, 0, 1, kHeadDim, dev);
     } else if (rest == "self_attn.o_proj.weight") {
       B200_REQUIRE(expect(H, QH), "shape mismatch for " + n);
       rc = copy_cols(w.wo, src, H, QH, r * ql, ql, dev);
@@ -1838,11 +1846,19 @@ int b200_engine_set_weight_fp8(b200_engine_t* e, const char* name, const void* d
 
 int b200_engine_finalize_weights(b200_engine_t* e) {
   B200_REQUIRE(e, "null engine");
-  // 3 + 9 L tensors, or 3 + 12 L when every layer also has its q / k / v projection biases (Qwen2); anything in between
-  // is refused: a layer without its bias would run silently wrong
-  size_t nbias = 0;
-  for (const auto& kv : e->seen)
-    if (kv.first.size() > 5 && kv.first.compare(kv.first.size() - 5, 5, ".bias") == 0) ++nbias;
+  // 3 + 9 L tensors, + 3 L when every layer also has its q / k / v projection biases (Qwen2), or + 2 L when every layer
+  // has its q / k norm weights (Qwen3); anything in between is refused (a layer without its bias or norm would run
+  // silently wrong), and so are biases together with norms, which no supported checkpoint has
+  auto ends_with = [](const std::string& a, const char* b) {
+    const size_t n = strlen(b);
+    return a.size() >= n && a.compare(a.size() - n, n, b) == 0;
+  };
+  size_t nbias = 0, nnorm = 0;
+  for (const auto& kv : e->seen) {
+    if (ends_with(kv.first, ".bias")) ++nbias;
+    if (ends_with(kv.first, "_norm.weight") && kv.first.find(".self_attn.") != std::string::npos) ++nnorm;
+  }
+  B200_REQUIRE(nbias == 0 || nnorm == 0, "q/k/v projection biases together with q/k norm weights are not supported");
   if (nbias > 0) {
     for (int l = 0; l < e->L; ++l)
       for (const char* pr : {"q", "k", "v"}) {
@@ -1850,7 +1866,14 @@ int b200_engine_finalize_weights(b200_engine_t* e) {
         B200_REQUIRE(e->seen.count(bn), "missing weight tensor " + bn + " (q/k/v projection biases must be given for every layer or for none)");
       }
   }
-  const size_t want = 3 + (size_t)e->L * (nbias > 0 ? 12 : 9);
+  if (nnorm > 0) {
+    for (int l = 0; l < e->L; ++l)
+      for (const char* pr : {"q", "k"}) {
+        const std::string nn = "model.layers." + std::to_string(l) + ".self_attn." + pr + "_norm.weight";
+        B200_REQUIRE(e->seen.count(nn), "missing weight tensor " + nn + " (q/k norm weights must be given for every layer or for none)");
+      }
+  }
+  const size_t want = 3 + (size_t)e->L * (9 + (nbias > 0 ? 3 : 0) + (nnorm > 0 ? 2 : 0));
   B200_REQUIRE(e->seen.size() == want, "expected " + std::to_string(want) + " weight tensors, got " + std::to_string(e->seen.size()));
   B200_CUDA_OK(cudaDeviceSynchronize());
   e->finalized = true;
@@ -2430,9 +2453,11 @@ static int op_attn_decode_fused(const void* qkv, int64_t ld_qkv, const float* qk
                                 int64_t ld_partial, const void* qkv_bias, const void* cos_tab, const void* sin_tab, void* out,
                                 int64_t ldo, void* kcache, void* vcache, const int32_t* page_table, int max_pages,
                                 const int32_t* seq_slot, const int32_t* tok_pos, int B, int nh, int nkv, int splits, float* part_o,
-                                float* part_ml, int32_t* split_counter, void* stream, bool kv8) {
+                                float* part_ml, int32_t* split_counter, void* stream, bool kv8,
+                                const void* q_norm_w = nullptr, const void* k_norm_w = nullptr, float qk_eps = 0.f) {
   B200_REQUIRE((qkv == nullptr) != (qkv_partial == nullptr), "exactly one of qkv / qkv_partial must be given");
   B200_REQUIRE(qkv_bias == nullptr || qkv_partial != nullptr, "qkv_bias applies to split-K partials only");
+  B200_REQUIRE((q_norm_w == nullptr) == (k_norm_w == nullptr), "q/k norm: both weights or neither");
   AttnDecodeParams p{};
   p.out = (bf16*)out; p.ldo = ldo; p.kcache = (const bf16*)kcache; p.vcache = (const bf16*)vcache;
   p.page_table = page_table; p.max_pages = max_pages; p.seq_slot = seq_slot; p.tok_pos = tok_pos; p.nh = nh; p.nkv = nkv;
@@ -2443,7 +2468,19 @@ static int op_attn_decode_fused(const void* qkv, int64_t ld_qkv, const float* qk
   p.qkv_bias = (const bf16*)qkv_bias; p.cos_tab = (const bf16*)cos_tab; p.sin_tab = (const bf16*)sin_tab;
   p.kcache_w = (bf16*)kcache; p.vcache_w = (bf16*)vcache;
   p.split_counter = split_counter;
+  p.q_norm_w = (const bf16*)q_norm_w; p.k_norm_w = (const bf16*)k_norm_w; p.qk_eps = qk_eps;
   return launch_attn_decode(p, B, (cudaStream_t)stream, kv8);
+}
+
+int b200_op_attn_decode_fused_norm(const void* qkv, int64_t ld_qkv, const float* qkv_partial, int qkv_splits,
+                                   int64_t split_stride, int64_t ld_partial, const void* qkv_bias, const void* q_norm_w,
+                                   const void* k_norm_w, float eps, const void* cos_tab, const void* sin_tab, void* out,
+                                   int64_t ldo, void* kcache, void* vcache, int kv8, const int32_t* page_table, int max_pages,
+                                   const int32_t* seq_slot, const int32_t* tok_pos, int B, int nh, int nkv, int splits,
+                                   float* part_o, float* part_ml, int32_t* split_counter, void* stream) {
+  return op_attn_decode_fused(qkv, ld_qkv, qkv_partial, qkv_splits, split_stride, ld_partial, qkv_bias, cos_tab, sin_tab, out, ldo,
+                              kcache, vcache, page_table, max_pages, seq_slot, tok_pos, B, nh, nkv, splits, part_o, part_ml,
+                              split_counter, stream, kv8 != 0, q_norm_w, k_norm_w, eps);
 }
 
 int b200_op_attn_decode_fused(const void* qkv, int64_t ld_qkv, const float* qkv_partial, int qkv_splits, int64_t split_stride,
@@ -2478,6 +2515,43 @@ int b200_op_rope_kv(const void* qkv, int64_t ld, void* q_out, int64_t ldq, void*
   rope_kv_kernel<false><<<(T + p.tokens_per_cta - 1) / p.tokens_per_cta, 512, 0, (cudaStream_t)stream>>>(p);
   B200_CUDA_OK(cudaGetLastError());
   return 0;
+}
+
+int b200_op_rope_kv_norm(const void* qkv, int64_t ld, void* q_out, int64_t ldq, void* kcache, void* vcache, int kv8,
+                         const int32_t* page_table, int max_pages, const int32_t* tok_seq, const int32_t* tok_pos,
+                         const void* cos_tab, const void* sin_tab, const void* q_norm_w, const void* k_norm_w, float eps,
+                         int T, int nh, int nkv, void* stream) {
+  B200_REQUIRE((q_norm_w == nullptr) == (k_norm_w == nullptr), "q/k norm: both weights or neither");
+  RopeKvParams p{};
+  p.qkv = (const bf16*)qkv; p.ld = ld; p.q_out = (bf16*)q_out; p.ldq = ldq; p.kcache = (bf16*)kcache; p.vcache = (bf16*)vcache;
+  p.page_table = page_table; p.max_pages = max_pages; p.tok_seq = tok_seq; p.tok_pos = tok_pos;
+  p.cos_tab = (const bf16*)cos_tab; p.sin_tab = (const bf16*)sin_tab; p.nh = nh; p.nkv = nkv;
+  p.q_norm_w = (const bf16*)q_norm_w; p.k_norm_w = (const bf16*)k_norm_w; p.qk_eps = eps;
+  p.T = T; p.tokens_per_cta = 1;
+  if (T <= 0) return 0;
+  if (kv8) rope_kv_kernel<true><<<T, 512, 0, (cudaStream_t)stream>>>(p);
+  else rope_kv_kernel<false><<<T, 512, 0, (cudaStream_t)stream>>>(p);
+  B200_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int b200_op_qkv_rope_kv(const void* x, const void* wqkv, void* out, int64_t ldo, int T, int H, int nh, int nkv,
+                        const void* bias, const void* q_norm_w, const void* k_norm_w, float eps, void* kcache, void* vcache,
+                        int kv8, const int32_t* page_table, int max_pages, const int32_t* tok_seq, const int32_t* tok_pos,
+                        const void* cos_tab, const void* sin_tab, void* stream) {
+  B200_REQUIRE((q_norm_w == nullptr) == (k_norm_w == nullptr), "q/k norm: both weights or neither");
+  g_op_tmaps.maps.clear();  // caller buffers may be reused at other shapes
+  const int N = (nh + 2 * nkv) * kHeadDim;
+  RopeKvParams rp{};
+  rp.qkv = (const bf16*)out; rp.ld = ldo; rp.q_out = (bf16*)out; rp.ldq = ldo;
+  rp.tok_seq = tok_seq; rp.tok_pos = tok_pos; rp.kcache = (bf16*)kcache; rp.vcache = (bf16*)vcache;
+  rp.page_table = page_table; rp.max_pages = max_pages; rp.cos_tab = (const bf16*)cos_tab; rp.sin_tab = (const bf16*)sin_tab;
+  rp.nh = nh; rp.nkv = nkv; rp.kv8 = kv8 != 0;
+  rp.q_norm_w = (const bf16*)q_norm_w; rp.k_norm_w = (const bf16*)k_norm_w; rp.qk_eps = eps;
+  GemmArgs a{(const bf16*)x, T, (const bf16*)wqkv, N, T, N, H, EPI_ROPE_KV, 256, 1, out, nullptr, ldo, 0, 0, false};
+  a.rope = &rp;
+  a.bias = (const bf16*)bias;
+  return launch_gemm(g_op_tmaps, a, op_sms(), (cudaStream_t)stream);
 }
 
 int b200_op_argmax(const void* logits, int64_t ld, int B, int V, float* out_val, int32_t* out_idx, void* stream) {

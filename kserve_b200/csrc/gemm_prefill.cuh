@@ -63,13 +63,16 @@ __device__ __forceinline__ float2 ld_bias2(const bf16* b, int col, int N) {
 // BIAS (EPI_STORE, EPI_ROPE_KV): add p.bias[column] to the fp32 accumulator before its bf16 rounding; a compile-time
 // flag, so the GEMMs without a bias run exactly the code they ran before.
 // KV8 (EPI_ROPE_KV): the paged cache holds e4m3 codes; each k / v row goes out as e4m3(bf16 value), 8 codes per store.
-template <int EPI, bool BIAS = false, bool KV8 = false>
+// QKNORM (EPI_ROPE_KV, no bias): Qwen3's per-head RMSNorm of q and k (p.rope_q_norm / p.rope_k_norm) between the
+// projection's bf16 rounding and RoPE, in common.cuh's qknorm order; a compile-time flag like BIAS.
+template <int EPI, bool BIAS = false, bool KV8 = false, bool QKNORM = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_prefill_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                     const __grid_constant__ CUtensorMap tmap_out, const GemmParams p) {
   static_assert(EPI == EPI_STORE || EPI == EPI_STORE_RES || EPI == EPI_SWIGLU || EPI == EPI_ROPE_KV, "row-major epilogues only");
   static_assert(!BIAS || EPI == EPI_STORE || EPI == EPI_ROPE_KV, "bias: QKV epilogues only");
   static_assert(!KV8 || EPI == EPI_ROPE_KV, "FP8 KV cache: the RoPE + KV epilogue only");
+  static_assert(!QKNORM || (EPI == EPI_ROPE_KV && !BIAS), "q/k norm: the RoPE + KV epilogue, without a projection bias");
   TraceScope _ts(TK_GEMM + 100 * EPI + 1000 * (p.M >> 7));
   using Cfg = PrefillCfg<EPI>;
   constexpr int STAGES = Cfg::kStages;
@@ -245,6 +248,40 @@ gemm_prefill_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
             }
           }
         } else {                                  // q or k head: rotate-half RoPE on the pairs (d, d + 64)
+          if constexpr (QKNORM) {
+            // this thread holds dims 8j + 2qd + {0, 1} (j = 0..15) of rows frag_row and frag_row + 8 of the head: round
+            // them to bf16, sum their squares in qknorm order, finish each row's sum across the quad, normalise in place
+            const bf16* nw = head < p.rope_nh ? p.rope_q_norm : p.rope_k_norm;
+            float ss[2] = {0.f, 0.f};
+#pragma unroll
+            for (int jl = 0; jl < 16; ++jl) {
+              const int j = 16 * hh + jl;
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                accum[4 * j + 2 * h] = bf16_round(accum[4 * j + 2 * h]);
+                accum[4 * j + 2 * h + 1] = bf16_round(accum[4 * j + 2 * h + 1]);
+                ss[h] = qknorm_acc(ss[h], accum[4 * j + 2 * h], accum[4 * j + 2 * h + 1]);
+              }
+            }
+            float rs[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float sh = ss[h];
+              sh += __shfl_xor_sync(0xffffffffu, sh, 1);
+              sh += __shfl_xor_sync(0xffffffffu, sh, 2);
+              rs[h] = qknorm_rstd(sh, p.rope_qk_eps);
+            }
+#pragma unroll
+            for (int jl = 0; jl < 16; ++jl) {
+              const int j = 16 * hh + jl;
+              const float2 wv = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(nw + 8 * jl + 2 * qd));
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                accum[4 * j + 2 * h] = qknorm_apply(accum[4 * j + 2 * h], rs[h], wv.x);
+                accum[4 * j + 2 * h + 1] = qknorm_apply(accum[4 * j + 2 * h + 1], rs[h], wv.y);
+              }
+            }
+          }
 #pragma unroll
           for (int jj = 0; jj < 8; ++jj) {
             const int j1 = 16 * hh + jj, j2 = j1 + 8;

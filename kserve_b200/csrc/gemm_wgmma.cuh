@@ -63,6 +63,7 @@ struct GemmParams {
   bf16* rope_kcache; bf16* rope_vcache;                      // this layer's [page][kv_head][64][128] (KV8: e4m3 codes)
   const bf16* rope_cos; const bf16* rope_sin;                // [max_pos][64]
   int rope_nh, rope_nkv;
+  const bf16* rope_q_norm; const bf16* rope_k_norm; float rope_qk_eps;   // EPI_ROPE_KV<.., QKNORM>: Qwen3 q / k norm weights [128]
   int stream_out;          // row-major epilogues: cache-streaming output stores
   int out_tma;             // row-major epilogues: `out` is addressable by TMA (16-byte aligned base and row pitch)
   int sched;

@@ -151,10 +151,10 @@ inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_
   return cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
 }
 
-template <int EPI, bool BIAS = false, bool KV8 = false>
+template <int EPI, bool BIAS = false, bool KV8 = false, bool QKNORM = false>
 int launch_prefill_inst(const CUtensorMap* ta, const CUtensorMap* tb, const CUtensorMap* to, const GemmParams& p, int grid,
                         cudaStream_t s) {
-  auto kern = gemm_prefill_kernel<EPI, BIAS, KV8>;
+  auto kern = gemm_prefill_kernel<EPI, BIAS, KV8, QKNORM>;
   static bool configured = false;  // per instantiation
   if (!configured) {
     B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PrefillCfg<EPI>::kSmemBytes));
@@ -297,12 +297,18 @@ inline int launch_gemm(TmapCache& cache, const GemmArgs& a, int num_sms, cudaStr
   p.a_scale = a.a_scale;
   p.rope_tok_seq = nullptr; p.rope_tok_pos = nullptr; p.rope_page_table = nullptr; p.rope_max_pages = 0;
   p.rope_kcache = nullptr; p.rope_vcache = nullptr; p.rope_cos = nullptr; p.rope_sin = nullptr; p.rope_nh = 0; p.rope_nkv = 0;
+  p.rope_q_norm = nullptr; p.rope_k_norm = nullptr; p.rope_qk_eps = 0.f;
   if (a.epi == EPI_ROPE_KV) {
     B200_REQUIRE(a.block_n == 256 && a.rope && a.N == (a.rope->nh + 2 * a.rope->nkv) * kHeadDim,
                  "EPI_ROPE_KV is the prefill QKV projection with 256-column tiles");
     p.rope_tok_seq = a.rope->tok_seq; p.rope_tok_pos = a.rope->tok_pos; p.rope_page_table = a.rope->page_table;
     p.rope_max_pages = a.rope->max_pages; p.rope_kcache = a.rope->kcache; p.rope_vcache = a.rope->vcache;
     p.rope_cos = a.rope->cos_tab; p.rope_sin = a.rope->sin_tab; p.rope_nh = a.rope->nh; p.rope_nkv = a.rope->nkv;
+    B200_REQUIRE((a.rope->q_norm_w == nullptr) == (a.rope->k_norm_w == nullptr) && (!a.rope->q_norm_w || !a.bias),
+                 "q/k norm: both weights or neither, and no projection bias with them");
+    B200_REQUIRE(((reinterpret_cast<uintptr_t>(a.rope->q_norm_w) | reinterpret_cast<uintptr_t>(a.rope->k_norm_w)) & 3) == 0,
+                 "q/k norm weights must be 4-byte aligned");
+    p.rope_q_norm = a.rope->q_norm_w; p.rope_k_norm = a.rope->k_norm_w; p.rope_qk_eps = a.rope->qk_eps;
   }
   p.out_tma = 0;
   if (a.epi == EPI_STORE || a.epi == EPI_STORE_RES || a.epi == EPI_SWIGLU || a.epi == EPI_ROPE_KV) {
@@ -321,6 +327,8 @@ inline int launch_gemm(TmapCache& cache, const GemmArgs& a, int num_sms, cudaStr
                                           : launch_prefill_inst<EPI_STORE>(ta, tb, to, p, grid, s);
     if (a.epi == EPI_STORE_RES) return launch_prefill_inst<EPI_STORE_RES>(ta, tb, to, p, grid, s);
     if (a.epi == EPI_SWIGLU) return launch_prefill_inst<EPI_SWIGLU>(ta, tb, to, p, grid, s);
+    if (p.rope_q_norm) return a.rope->kv8 ? launch_prefill_inst<EPI_ROPE_KV, false, true, true>(ta, tb, to, p, grid, s)
+                                          : launch_prefill_inst<EPI_ROPE_KV, false, false, true>(ta, tb, to, p, grid, s);
     if (a.rope->kv8) return a.bias ? launch_prefill_inst<EPI_ROPE_KV, true, true>(ta, tb, to, p, grid, s)
                                    : launch_prefill_inst<EPI_ROPE_KV, false, true>(ta, tb, to, p, grid, s);
     return a.bias ? launch_prefill_inst<EPI_ROPE_KV, true>(ta, tb, to, p, grid, s)

@@ -264,6 +264,9 @@ struct RopeKvParams {
   int nh, nkv;
   int T, tokens_per_cta;                     // tokens in this launch; consecutive tokens handled by one CTA
   bool kv8;                                  // the caches hold e4m3 codes (rope_kv_kernel<true>, EPI_ROPE_KV's KV8 instantiation)
+  // Qwen3: per-head RMSNorm of q (q_norm_w) and k (k_norm_w), [128] each, before RoPE (common.cuh: qknorm_*); both
+  // nullptr = none
+  const bf16* q_norm_w; const bf16* k_norm_w; float qk_eps;
 };
 
 __device__ __forceinline__ void load8(const RopeKvParams& p, int t, int col, float (&f)[8]) {
@@ -313,6 +316,23 @@ __global__ void __launch_bounds__(512) rope_kv_kernel(const RopeKvParams p) {
       float x1[8], x2[8], cs[8], sn[8];
       load8(p, t, col + c, x1);
       load8(p, t, col + c + 64, x2);
+      if (p.q_norm_w) {   // the head's sum of squares in the fragment order of the fused epilogue: re-read the whole head
+        float ss[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll 1
+        for (int j = 0; j < 16; ++j) {
+          float f[8];
+          load8(p, t, col + 8 * j, f);
+#pragma unroll
+          for (int qd = 0; qd < 4; ++qd) ss[qd] = qknorm_acc(ss[qd], f[2 * qd], f[2 * qd + 1]);
+        }
+        const float r = qknorm_rstd(qknorm_sum(ss[0], ss[1], ss[2], ss[3]), p.qk_eps);
+        const bf16* w = head < p.nh ? p.q_norm_w : p.k_norm_w;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          x1[i] = qknorm_apply(x1[i], r, __bfloat162float(w[c + i]));
+          x2[i] = qknorm_apply(x2[i], r, __bfloat162float(w[c + 64 + i]));
+        }
+      }
       {
         uint4 cu = *reinterpret_cast<const uint4*>(p.cos_tab + (long long)pos * 64 + c);
         uint4 su = *reinterpret_cast<const uint4*>(p.sin_tab + (long long)pos * 64 + c);

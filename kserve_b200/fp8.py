@@ -76,7 +76,9 @@ def parse_quantization_config(cfg: Dict[str, Any], tp_size: int = 1) -> Optional
         return None
     method = qc.get("quant_method")
     if method != "compressed-tensors":
-        _refuse(f"quantization_config.quant_method={method!r} is not supported")
+        blocks = qc.get("weight_block_size")   # quant_method "fp8" with 128 x 128 blocks: the official Qwen3-*-FP8 checkpoints
+        _refuse(f"quantization_config.quant_method={method!r} is not supported"
+                + (f" (block-scaled FP8, weight_block_size={blocks})" if blocks else ""))
     if qc.get("format") != "float-quantized":
         _refuse(f"quantization_config.format={qc.get('format')!r} is not supported")
     if qc.get("kv_cache_scheme"):
@@ -100,7 +102,8 @@ def parse_quantization_config(cfg: Dict[str, Any], tp_size: int = 1) -> Optional
         if not w.get("symmetric", False) or w.get("dynamic"):
             _refuse(f"config group {gname}: asymmetric or dynamic weight quantization is not supported")
         if w.get("strategy") not in ("channel", "tensor"):
-            _refuse(f"config group {gname}: weight strategy={w.get('strategy')!r} (block / group scales) is not supported")
+            _refuse(f"config group {gname}: weight strategy={w.get('strategy')!r} (block / group scales, e.g. the official "
+                    "Qwen3-*-FP8 checkpoints' 128x128 blocks) is not supported")
         strategies.add(w["strategy"])
         if g.get("output_activations"):
             _refuse(f"config group {gname}: output activation quantization is not supported")

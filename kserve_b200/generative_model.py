@@ -155,9 +155,10 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
         cfg = self.model_config
         arch = (cfg.get("architectures") or ["LlamaForCausalLM"])[0]
         model_type = cfg.get("model_type", "llama")
-        if not arch.endswith("ForCausalLM") or model_type not in ("llama", "mistral", "mixtral", "qwen2"):
-            raise OpenAIError(f"architecture {arch} is not supported by the H100 runtime "
-                              "(Llama / Mistral / Mixtral / Qwen2 decoders only)")
+        # (Qwen3 = the dense decoders; qwen3_moe and the other qwen3_* types are different models)
+        if not arch.endswith("ForCausalLM") or model_type not in ("llama", "mistral", "mixtral", "qwen2", "qwen3"):
+            raise OpenAIError(f"architecture {arch} (model_type {model_type}) is not supported by the H100 runtime "
+                              "(Llama / Mistral / Mixtral / Qwen2 / dense Qwen3 decoders only)")
         head_dim = cfg.get("head_dim") or cfg["hidden_size"] // cfg["num_attention_heads"]
         if head_dim != 128:
             # (Qwen2-0.5B, Qwen2.5-0.5B, Llama-3.2-1B: the KV page layout and both attention kernels are built for 128)
@@ -191,8 +192,8 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
             logger.warning("sliding_window=%d < max length %d: serving at most %d tokens (full attention == sliding "
                            "window inside the window)", window, self.max_length, window)
             self.max_length = int(window)
-        # Qwen2's q / k / v biases are implied by its architecture (they come with the checkpoint); a Llama
-        # attention_bias would also put one on o_proj, which the engine does not have
+        # Qwen2's q / k / v biases and Qwen3's q / k norms are implied by the architecture (they come with the
+        # checkpoint); attention_bias (Llama, Qwen3) would also put a bias on o_proj, which the engine does not have
         for key in ("attention_bias", "mlp_bias"):
             if cfg.get(key):
                 raise OpenAIError(f"config.{key}=true is not supported by the H100 runtime")
@@ -244,9 +245,14 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
 
         tied: List[Optional[torch.Tensor]] = [None]
         seen_head = [False]
+        # Qwen3: the engine applies the per-head q / k norms when their weights arrive, so a checkpoint without them would
+        # run as a plain Llama decoder and generate wrong tokens; they must be there for every layer
+        qk_norms = {f"model.layers.{i}.self_attn.{p}_norm.weight" for i in range(cfg["num_hidden_layers"]) for p in "qk"} \
+            if model_type == "qwen3" else set()
 
         def resized():
             for name, t in weights:
+                qk_norms.discard(name)
                 if name in ("model.embed_tokens.weight", "lm_head.weight") and t.shape[0] != vocab_rows:
                     # resize_token_embeddings: keep the first rows, new rows = mean of the old ones (HF default)
                     if t.shape[0] > vocab_rows:
@@ -259,6 +265,9 @@ class B200GenerativeModel(OpenAIChatAdapterModel, Model):
                 if name == "lm_head.weight":
                     seen_head[0] = True
                 yield name, t
+            if qk_norms:
+                raise OpenAIError(f"the qwen3 checkpoint has no {min(qk_norms)}: a Qwen3 decoder without its per-head q / k "
+                                  "norms is not supported by the H100 runtime")
             # tie_word_embeddings: the checkpoint has no lm_head.weight; the head IS the (resized) embedding matrix
             if cfg.get("tie_word_embeddings") and not seen_head[0]:
                 if tied[0] is None:

@@ -1,6 +1,7 @@
 """Llama-family tensor table: HF state_dict names and shapes the engine expects
 (what AutoModelForCausalLM.from_pretrained loads in the reference, generative_model.py:249-254).
-Qwen2 configs (model_type "qwen2") add the q / k / v projection biases, and a tied checkpoint has no lm_head.weight."""
+Qwen2 configs (model_type "qwen2") add the q / k / v projection biases, Qwen3 configs (model_type "qwen3") the per-head
+q / k norm weights, and a tied checkpoint has no lm_head.weight."""
 from __future__ import annotations
 
 from typing import Iterator, Tuple
@@ -13,6 +14,7 @@ def llama_tensor_specs(cfg: dict) -> Iterator[Tuple[str, Tuple[int, ...], str]]:
     d = cfg.get("head_dim") or H // nh
     E = int(cfg.get("num_local_experts", 0) or 0)
     qwen2 = cfg.get("model_type") == "qwen2"
+    qwen3 = cfg.get("model_type") == "qwen3"
     yield "model.embed_tokens.weight", (V, H), "embed"
     for i in range(cfg["num_hidden_layers"]):
         if E:   # Mixtral-style sparse MoE (transformers 5.x fused-expert state_dict)
@@ -35,6 +37,9 @@ def llama_tensor_specs(cfg: dict) -> Iterator[Tuple[str, Tuple[int, ...], str]]:
         yield p + "self_attn.k_proj.weight", (nkv * d, H), "linear"
         if qwen2:
             yield p + "self_attn.k_proj.bias", (nkv * d,), "bias"
+        if qwen3:
+            yield p + "self_attn.q_norm.weight", (d,), "norm"
+            yield p + "self_attn.k_norm.weight", (d,), "norm"
         yield p + "self_attn.v_proj.weight", (nkv * d, H), "linear"
         if qwen2:
             yield p + "self_attn.v_proj.bias", (nkv * d,), "bias"

@@ -1,6 +1,7 @@
 """Throughput of one served model family on synthetic weights, timed the way bench.py times Llama-3-8B.
 
     python tools/model_bench.py                       # Qwen2.5-7B dims (28 layers), batch 32, 1024-in / 128-out
+    python tools/model_bench.py --model qwen3_8b              # Qwen3-8B dims (36 layers, per-head q / k norms)
     python tools/model_bench.py --model llama3_8b --steps 3
     python tools/model_bench.py --model llama3_8b --weights fp8       # FP8 projections (e4m3 + a bf16 scale per row)
     python tools/model_bench.py --model llama3_8b --kv-cache fp8      # FP8 KV cache (one e4m3 code per K / V element)

@@ -67,14 +67,15 @@ def build_model(cfg: dict, state_dict, dtype=torch.bfloat16):
 ONLY = None         # --only: the case names to (re)generate
 
 
-def gen_case(name, cfg_name, seed, prompt, max_tokens, pad_token_id, sub_logits=False):
+def gen_case(name, cfg_name, seed, prompt, max_tokens, pad_token_id, sub_logits=False, build=None):
     """greedy generate of the oracle with every step's logits -> tests/golden/<name>.npz (full logits, or for a big
-    vocabulary the logits on make_goldens.sub_columns + the top-16)"""
+    vocabulary the logits on make_goldens.sub_columns + the top-16); `build` (config, state dict) -> model, default
+    build_model"""
     if ONLY is not None and name not in ONLY:
         return
     cfg = W.CONFIGS[cfg_name]
     sd = W.synth_state_dict(cfg, seed)
-    model = build_model(cfg, sd)
+    model = (build or build_model)(cfg, sd)
     orc = OracleGenerativeModel(model, pad_token_id=pad_token_id)
     res = orc.create_completion(prompt, max_tokens=max_tokens, stop=(), temperature=0, want_logits=True)
     tv, ti = topk_pack(res.step_logits)

@@ -96,6 +96,33 @@ for _base in ("tiny_qwen2", "qwen2_7b_2l"):
     QWEN2_CONFIGS[_base + "_peaked"] = dict(QWEN2_CONFIGS[_base], _peaked=True)
 CONFIGS.update(QWEN2_CONFIGS)
 
+# Qwen3 dense decoders: Llama layers plus a per-head RMSNorm of q and of k (q_norm / k_norm, [128] each) before RoPE, no
+# projection biases, theta 1e6, eps 1e-6.  tiny_qwen3 has 0.6B's q dim = 2H, G = 2 and tied embeddings, and its decode
+# QKV projection (16 m-tiles) takes split-K; g4 / g5 are 8B's and 14B's groups; tiny_qwen3_wide (G = 8, qkv_cols 10240
+# = 80 m-tiles) takes the bf16 EPI_T_STORE decode epilogue, as the 32B class does.
+_QWEN3 = dict(model_type="qwen3", head_dim=128, max_position_embeddings=2048, rms_norm_eps=1e-6, rope_theta=1000000.0,
+              use_sliding_window=False)
+QWEN3_CONFIGS: Dict[str, dict] = {
+    "tiny_qwen3": dict(_QWEN3, vocab_size=1031, hidden_size=512, intermediate_size=1536, num_hidden_layers=2,
+                       num_attention_heads=8, num_key_value_heads=4, tie_word_embeddings=True),
+    "tiny_qwen3_g4": dict(_QWEN3, vocab_size=1031, hidden_size=1024, intermediate_size=2048, num_hidden_layers=2,
+                          num_attention_heads=8, num_key_value_heads=2),
+    "tiny_qwen3_g5": dict(_QWEN3, vocab_size=1031, hidden_size=640, intermediate_size=1536, num_hidden_layers=2,
+                          num_attention_heads=10, num_key_value_heads=2),
+    "tiny_qwen3_wide": dict(_QWEN3, vocab_size=1031, hidden_size=512, intermediate_size=1024, num_hidden_layers=2,
+                            num_attention_heads=64, num_key_value_heads=8),
+    # Qwen3-8B layer and vocabulary shapes, 2 layers
+    "qwen3_8b_2l": dict(_QWEN3, vocab_size=151936, hidden_size=4096, intermediate_size=12288, num_hidden_layers=2,
+                        num_attention_heads=32, num_key_value_heads=8, max_position_embeddings=40960),
+    # Qwen3-8B, all 36 layers (tools/model_bench.py)
+    "qwen3_8b": dict(_QWEN3, vocab_size=151936, hidden_size=4096, intermediate_size=12288, num_hidden_layers=36,
+                     num_attention_heads=32, num_key_value_heads=8, max_position_embeddings=40960),
+}
+# (a peaked head is a permuted embedding, so the peaked tiny case is untied)
+QWEN3_CONFIGS["tiny_qwen3_peaked"] = dict(QWEN3_CONFIGS["tiny_qwen3"], tie_word_embeddings=False, _peaked=True)
+QWEN3_CONFIGS["qwen3_8b_2l_peaked"] = dict(QWEN3_CONFIGS["qwen3_8b_2l"], _peaked=True)
+CONFIGS.update(QWEN3_CONFIGS)
+
 # FP8 checkpoints (compressed-tensors float-quantized, kserve_b200/fp8.py): the SAME seeded bf16 tensors as the base
 # config, each q/k/v/o/gate/up/down projection quantized to float8_e4m3fn with a scale amax / 448 per row ("channel") or
 # per tensor ("tensor"), in bf16 or fp32; everything else (embeddings, norms, lm_head, Qwen2 biases) stays bf16.
@@ -108,6 +135,7 @@ FP8_CONFIGS: Dict[str, dict] = {
     "tiny_qwen2_g6_tied_fp8": dict(CONFIGS["tiny_qwen2_g6_tied"], _fp8="channel", _fp8_scale="float32"),
     "llama3_8b_2l_fp8": dict(CONFIGS["llama3_8b_2l"], _fp8="channel"),
     "llama3_8b_2l_fp8_peaked": dict(CONFIGS["llama3_8b_2l_peaked"], _fp8="channel"),
+    "tiny_qwen3_fp8": dict(CONFIGS["tiny_qwen3"], _fp8="channel"),                               # q/k norms, tied, G = 2
 }
 CONFIGS.update(FP8_CONFIGS)
 FP8_PROJECTIONS = ("self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight", "self_attn.o_proj.weight",
@@ -159,13 +187,15 @@ def moe_tensor_specs(cfg: dict) -> Iterator[Tuple[str, Tuple[int, ...], str]]:
 
 def tensor_specs(cfg: dict) -> Iterator[Tuple[str, Tuple[int, ...], str]]:
     """Yield (name, shape, kind) in canonical order. kind in {embed, linear, norm, bias}.  Qwen2 biases follow their
-    weight, and a tied checkpoint has no lm_head.weight; the Llama / Mixtral order (and so every seed) is unchanged."""
+    weight, Qwen3's q_norm / k_norm follow k_proj, and a tied checkpoint has no lm_head.weight; the Llama / Mixtral order
+    (and so every seed) is unchanged."""
     H, I, V = cfg["hidden_size"], cfg["intermediate_size"], cfg["vocab_size"]
     nh, nkv, d = cfg["num_attention_heads"], cfg["num_key_value_heads"], cfg["head_dim"]
     if "num_local_experts" in cfg:
         yield from moe_tensor_specs(cfg)
         return
     qwen2 = cfg.get("model_type") == "qwen2"
+    qwen3 = cfg.get("model_type") == "qwen3"
     yield "model.embed_tokens.weight", (V, H), "embed"
     for i in range(cfg["num_hidden_layers"]):
         p = f"model.layers.{i}."
@@ -174,6 +204,9 @@ def tensor_specs(cfg: dict) -> Iterator[Tuple[str, Tuple[int, ...], str]]:
             yield p + f"self_attn.{proj}_proj.weight", (rows, H), "linear"
             if qwen2:
                 yield p + f"self_attn.{proj}_proj.bias", (rows,), "bias"
+            if qwen3 and proj == "k":
+                yield p + "self_attn.q_norm.weight", (d,), "norm"
+                yield p + "self_attn.k_norm.weight", (d,), "norm"
         yield p + "self_attn.o_proj.weight", (H, nh * d), "linear"
         yield p + "post_attention_layernorm.weight", (H,), "norm"
         yield p + "mlp.gate_proj.weight", (I, H), "linear"
@@ -197,6 +230,23 @@ def synth_bias(index: int, shape, name: str, seed: int, dtype=torch.bfloat16) ->
     else:
         t = 0.5 * torch.randn(shape, generator=g, dtype=torch.float32)
     return t.to(dtype)
+
+
+def synth_qk_norm(index: int, shape, name: str, seed: int, dtype=torch.bfloat16) -> torch.Tensor:
+    """Qwen3 q_norm / k_norm weights.  HF initialises them to ones, so they are drawn far from 1 (log-uniform over
+    [0.2, 4]) that a dropped, post-RoPE or swapped norm moves the logits; k_norm also gets two entries near +-10..20, the
+    outliers real Qwen3 k_norm weights have."""
+    g = torch.Generator(device="cpu")
+    g.manual_seed(seed * 1000003 + index * 7919 + 17)
+    t = torch.exp(math.log(0.2) + (math.log(4.0) - math.log(0.2)) * torch.rand(shape, generator=g, dtype=torch.float32))
+    if ".k_norm." in name:
+        idx = torch.randperm(shape[0], generator=g)[:2]
+        t[idx] = torch.sign(torch.randn(idx.shape, generator=g)) * (10.0 + 10.0 * torch.rand(idx.shape, generator=g))
+    return t.to(dtype)
+
+
+# Qwen3 q / k projections: an RMS well away from 1 (the norm removes it; a dropped norm does not)
+QWEN3_QK_SCALE = {"self_attn.q_proj.weight": 3.0, "self_attn.k_proj.weight": 0.3}
 
 
 def synth_tensor(index: int, shape, kind: str, seed: int, dtype=torch.bfloat16) -> torch.Tensor:
@@ -240,6 +290,14 @@ def iter_state_dict(cfg: dict, seed: int = 0, dtype=torch.bfloat16):
         if kind == "bias":
             yield name, synth_bias(idx, shape, name, seed, dtype)
             continue
+        if cfg.get("model_type") == "qwen3":
+            if name.endswith(("self_attn.q_norm.weight", "self_attn.k_norm.weight")):
+                yield name, synth_qk_norm(idx, shape, name, seed, dtype)
+                continue
+            qk = QWEN3_QK_SCALE.get(name.split(".", 3)[-1])
+            if qk is not None:
+                yield name, (synth_tensor(idx, shape, kind, seed, torch.float32) * qk).to(dtype)
+                continue
         yield name, synth_tensor(idx, shape, kind, seed, dtype)
 
 
