@@ -353,6 +353,16 @@ int b200_cb_read(b200_engine_t* e, int32_t slot, int32_t first, int64_t* out, in
 int b200_cb_release(b200_engine_t* e, int32_t slot);
 int b200_cb_stats(b200_engine_t* e, int64_t* out10);
 int b200_cb_end(b200_engine_t* e);
+
+/* Logits tap of the continuous batcher (tests and diagnostics; tp_size must be 1).  buf: device bf16
+ * [max_batch][max_steps][vocab_size].  While set, every LM-head pass of the batcher — the head of a prefill pass that
+ * ends prompts and the head of each decode step — copies the bf16 logits of each row to buf[slot][n][:], where n is the
+ * index of the token the pass generates for that slot (0 = the prompt's first token), as long as n < max_steps.
+ * Finished sequences are not written.  A slot's rows are overwritten when the slot is reused, so read them before
+ * releasing it.  buf = NULL turns the tap off.  Setting or clearing it waits for the engine stream and drops the
+ * batcher's captured decode graphs (they hold the buffer pointer); with the tap off the batcher launches exactly the
+ * kernels it launches without this call. */
+int b200_cb_logits_tap(b200_engine_t* e, void* buf, int32_t max_steps);
 /* Host-DRAM KV tier (BASELINE.json configs[3]) for the continuous batcher: preempt a RUNNING sequence to pinned host memory
  * (all of its KV pages, asynchronously on the engine stream; its pages return to the pool, it leaves the decode batch, its
  * per-sequence state stays on the device) and bring it back later (fresh pages; rc -7 while the pool cannot supply them).

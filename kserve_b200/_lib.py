@@ -117,6 +117,7 @@ def load() -> C.CDLL:
     lib.b200_cb_read.argtypes = [vp, i32, i32, C.POINTER(C.c_int64), i32, C.POINTER(i32)]
     lib.b200_cb_release.argtypes = [vp, i32]
     lib.b200_cb_end.argtypes = [vp]
+    lib.b200_cb_logits_tap.argtypes = [vp, vp, i32]
     lib.b200_debug_trace.argtypes = [i32]
     lib.b200_debug_trace_read.argtypes = [vp, i32, C.POINTER(i32)]
     _lib = lib

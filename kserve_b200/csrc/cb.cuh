@@ -63,6 +63,22 @@ __global__ void cb_gather_kernel(const int32_t* __restrict__ row_slot, int R, Cb
   dec_pos[r] = st.len[slot];     // a finished slot keeps rewriting the same cache position: harmless, never read
 }
 
+// logits tap (b200_cb_logits_tap): one CTA per row copies the row's logits to buf[slot][n_gen[slot]], the step whose
+// token the step kernel is about to append, while that is below max_steps.  Runs between the LM-head GEMM and the
+// argmax / sample kernel, so n_gen has not advanced yet; finished slots (frozen rows of the decode pass) are skipped.
+__global__ void cb_tap_kernel(const bf16* __restrict__ logits, long long ld, int V, const int32_t* __restrict__ row_slot,
+                              CbState st, bf16* __restrict__ buf, int max_steps) {
+  TraceScope _ts(TK_OTHER);
+  pdl_launch_dependents();
+  pdl_wait();
+  const int slot = row_slot[blockIdx.x];
+  const int g = st.n_gen[slot];
+  if (st.finished[slot] || g >= max_steps) return;
+  const bf16* src = logits + (long long)blockIdx.x * ld;
+  bf16* dst = buf + ((long long)slot * max_steps + g) * V;
+  for (int i = threadIdx.x; i < V; i += blockDim.x) dst[i] = src[i];
+}
+
 // one thread per row: merge the argmax candidates, append the token, EOS / max_new / stop sequences per sequence.
 // use_p2p: tensor parallel — the vocab-parallel candidates of every rank arrive through peer memory (argmax_kernel
 // pushes them); every row merges them even when its slot is finished, so the exchange epochs stay in step on all ranks.

@@ -216,6 +216,8 @@ struct b200_engine {
   std::vector<char> cb_slot_sampling;    // slot uses the processed-score path
   int cb_sampling_slots = 0;
   int32_t* d_kv_off = nullptr;           // [80] tokens of each prefill row's sequence that are already cached
+  bf16* cb_tap = nullptr;                // b200_cb_logits_tap: [max_batch][cb_tap_steps][Vl] (caller's memory), null = off
+  int cb_tap_steps = 0;
   // weight-stream L2 prefetch (prefetch.cuh): the step's weight-streaming GEMMs in launch order, per graph key
   PfCtx pf;
   std::unordered_map<int, std::vector<PfGemm>> pf_tables;
@@ -712,6 +714,11 @@ static int head_and_step(b200_engine* e, const bf16* rows_xn, int rows_cap, int 
   GemmArgs a{e->lm_head, e->Vl, rows_xn, rows_cap, e->Vl, B, e->H, EPI_T_STORE, pick_block_n(B), 1,
              e->logits, nullptr, e->Vl, 0, 0, true};
   if ((rc = launch_gemm(e, a, e->num_sms, s))) return rc;
+  if (cb_row_slot && e->cb_tap) {
+    B200_CUDA_OK(launch_k(cb_tap_kernel, dim3(B), dim3(256), 0, s, (const bf16*)e->logits, (long long)e->Vl, e->Vl, cb_row_slot, e->cb,
+                          e->cb_tap, e->cb_tap_steps));
+    e->launches++;
+  }
   const int use_p2p = (e->cfg.tp_size > 1 && e->p2p_ready) ? 1 : 0;
   // one GPU: 16 CTAs per row scan slices of the 128k-entry row (a single CTA per row took 65 us of the 4.3 ms step)
   const int chunks = (e->cfg.tp_size == 1 && e->Vl >= 16384) ? 16 : 1;
@@ -1170,7 +1177,7 @@ static int cb_decode_step(b200_engine* e) {
   }
   static const bool eager = getenv("B200_NO_GRAPH") != nullptr;
   if (eager) return cb_decode_enqueue(e, R);
-  const int key = R | (1 << 20) | (e->cb_num_eos << 9) | (e->cb_sampling_slots > 0 ? 1 << 21 : 0);
+  const int key = R | (1 << 20) | (e->cb_num_eos << 9) | (e->cb_sampling_slots > 0 ? 1 << 21 : 0) | (e->cb_tap ? 1 << 22 : 0);
   return graph_step(e, key, [&] { return cb_decode_enqueue(e, R); });
 }
 
@@ -2098,6 +2105,28 @@ int b200_cb_config(b200_engine_t* e, int32_t prefill_chunk_tokens, int32_t prefi
   B200_REQUIRE(prefill_chunk_tokens == 0 || prefill_chunk_tokens >= 128, "prefill chunks are multiples of 128 tokens (0 = whole prompts at admit)");
   e->cb_chunk_tokens = (prefill_chunk_tokens / 128) * 128;
   e->cb_prefix_on = prefix_cache != 0;
+  return 0;
+}
+
+int b200_cb_logits_tap(b200_engine_t* e, void* buf, int32_t max_steps) {
+  B200_REQUIRE(e, "null engine");
+  B200_REQUIRE(e->cfg.tp_size == 1, "the logits tap needs the whole vocabulary on one GPU (tp_size == 1)");
+  B200_REQUIRE(!buf || max_steps >= 1, "max_steps must be >= 1");
+  B200_CUDA_OK(cudaSetDevice(e->cfg.device));
+  B200_CUDA_OK(cudaStreamSynchronize(e->stream));     // nothing queued still writes to the previous buffer
+  // the decode graphs of the batcher have the tap's pointer and step count baked in: drop them all
+  for (auto it = e->graphs.begin(); it != e->graphs.end();) {
+    if (it->first & (1 << 20)) {
+      cudaGraphExecDestroy(it->second);
+      e->graph_nodes.erase(it->first);
+      e->pf_tables.erase(it->first);
+      it = e->graphs.erase(it);
+    } else {
+      ++it;
+    }
+  }
+  e->cb_tap = reinterpret_cast<bf16*>(buf);
+  e->cb_tap_steps = buf ? max_steps : 0;
   return 0;
 }
 

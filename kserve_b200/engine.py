@@ -384,6 +384,20 @@ class B200Engine:
     def cb_end(self) -> None:
         _lib.check(self.lib.b200_cb_end(self.h), "b200_cb_end")
 
+    def cb_logits_tap(self, max_steps: int) -> Optional[torch.Tensor]:
+        """Turn on the batcher's logits tap (include/kserve_b200.h: b200_cb_logits_tap) and return its device buffer,
+        bf16 [max_batch, max_steps, vocab] filled with NaN: row [s, n] receives the logits from which slot s's n-th
+        generated token was chosen.  max_steps 0 turns the tap off and returns None."""
+        buf = None
+        if max_steps > 0:
+            buf = torch.full((self.max_batch, int(max_steps), self.vocab), float("nan"), dtype=torch.bfloat16,
+                             device=torch.device("cuda", self.device))
+            torch.cuda.synchronize(buf.device)
+        _lib.check(self.lib.b200_cb_logits_tap(self.h, buf.data_ptr() if buf is not None else None, int(max_steps)),
+                   "b200_cb_logits_tap")
+        self._cb_tap = buf         # the engine writes into it until the tap is turned off or replaced
+        return buf
+
     def fetch_staged(self) -> torch.Tensor:
         B, S, T = self._staged_shape
         out = torch.empty((B, S + T), dtype=torch.int64)

@@ -28,6 +28,17 @@ def test_library_exports_every_declared_symbol(lib):
     assert b"sm_90a" in lib.b200_version()
 
 
+def test_batcher_entry_points_have_python_prototypes(lib):
+    """ctypes passes unprototyped pointer / int32 arguments as C ints: every b200_cb_* symbol the header declares
+    needs its argtypes in _lib.load()"""
+    from kserve_b200 import _lib
+    L = _lib.load()
+    cb = [s for s in _declared_symbols() if s.startswith("b200_cb_")]
+    assert "b200_cb_logits_tap" in cb
+    missing = [s for s in cb if getattr(L, s).argtypes is None]
+    assert not missing, f"no argtypes in kserve_b200/_lib.py: {missing}"
+
+
 def test_no_cpu_fallback(lib):
     """Without a CUDA device the engine refuses to exist (no CPU / oracle fallback in the product path)."""
     import torch
